@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the SegMamba hot path on B200.
+"""bench.py -- headline benchmark of the SegMamba hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W            # native arm (one rank per GPU under torchrun for N > 1)
     python bench.py --impl reference --gpus N --steps K --warmup W   # CPU arm: the oracle port on the host cores
@@ -56,6 +56,10 @@ def parse_args():
     ap.add_argument("--no-ref-cuda", action="store_true",
                     help="skip the vs_ref_cuda leg (reference op sequence on the reference's CUDA kernels from oracle/_ref)")
     ap.add_argument("--ref-cuda-steps", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the last timed step computed (loss, logits, updated parameters) as DIR/<name>.npy (float32; an output of more "
+                         "than 2^20 elements as a fixed seeded sample).  Inputs and weights are seeded, so two builds can be compared "
+                         "output for output")
     return ap.parse_args()
 
 
@@ -227,14 +231,22 @@ def scan_bwd_bytes(meta):
     return s * batch * L * (streams * dim + 2 * N) + 2 * 4 * batch * N * L + 4 * batch * (nck + 1) * N * dim
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per call (all passes of the op) from the committed `ncu --set full` capture of this
-# round, keyed by (op, batch, dim, L, N, element bytes).  Constants from a profiler run of the same kernels (tools/profile_step.py
-# --what scan), not measured by this script; a launch whose key is not listed reports traffic null.
-NCU_DRAM_SOURCE = "profiles/r2l_ncu_scan_summary.txt (ncu --set full, slot r2l: agg2 + main2 forward; ragg2 + main2<dense> backward)"
-NCU_DRAM_BYTES = {
-    ("scan_fwd", 2, 96, 262144, 16, 2): int((218.3 + 16.28 + 352.9 + 463.1) * 1e6),     # incl. the 402 MB dense checkpoint write
-    ("scan_bwd", 2, 96, 262144, 16, 2): int((320.0 + 362.8 + 1316.0 + 357.9) * 1e6),    # incl. dense checkpoints: mdense write, hdense + mdense reads
-}
+DUMP_CAP = 1 << 20      # elements kept per dumped output
+
+
+def dump_outputs(directory, arrays):
+    """--dump-outputs: one float32 .npy per named tensor; a tensor above DUMP_CAP elements is sampled at positions drawn once from a
+    fixed seed, so the same positions are kept in every run."""
+    import numpy as np
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_CAP:
+            idx = torch.randint(0, flat.numel(), (DUMP_CAP,), generator=torch.Generator().manual_seed(1234)).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(directory, name + ".npy"), flat.float().cpu().numpy())
+
 
 _T0 = time.time()
 
@@ -271,7 +283,7 @@ def _start_stall_watchdog(rank, limit_s=420.0):
 def run_ref_cuda_leg(args, native_ms_per_step, log):
     """The denominator of north_star's ">= 5x the reference CUDA path": the reference's op sequence (NCDHW, flips / stack /
     rearrange copies, ATen InstanceNorm3d / LayerNorm, cuDNN / cuBLAS as the reference calls them) on the reference's OWN CUDA
-    kernels compiled for sm_100a (oracle/_ref/*.so, oracle/build_ref.py), same patch / batch / bf16 autocast / optimizer, timed
+    kernels compiled for sm_90a (oracle/_ref/*.so, oracle/build_ref.py), same patch / batch / bf16 autocast / optimizer, timed
     on the same GPU right after the native arm's timed region.  Baseline only: nothing here is on the product path."""
     import gc
     import importlib.util
@@ -281,11 +293,12 @@ def run_ref_cuda_leg(args, native_ms_per_step, log):
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
         if not os.path.exists(os.path.join(ROOT, "oracle", "_ref", "selective_scan_cuda.so")):
-            return {"unavailable": "oracle/_ref/*.so not built (python oracle/build_ref.py in the build container)"}
+            return {"unavailable": "oracle/_ref/*.so not built (python oracle/build_ref.py where the reference sources are present)"}
         gc.collect()
         torch.cuda.empty_cache()
         log(0, "vs_ref_cuda leg: reference op sequence on the reference CUDA kernels")
         ref_step, params = mod.make_ref_step(args.batch, args.patch, "cuda")
+        torch.backends.cudnn.benchmark = False                     # make_ref_step switches autotuning on; both arms run without it
         for _ in range(2):
             ref_step()
         torch.cuda.synchronize()
@@ -298,7 +311,7 @@ def run_ref_cuda_leg(args, native_ms_per_step, log):
         ref_ms = s.elapsed_time(e) / args.ref_cuda_steps
         out = {"ref_ms_per_step": ref_ms, "ref_patches_per_s": args.batch / (ref_ms / 1e3), "native_ms_per_step": native_ms_per_step,
                "ratio": ref_ms / native_ms_per_step, "steps": args.ref_cuda_steps, "ref_loss": float(loss.detach()),
-               "kind": "reference CUDA ext (selective_scan_cuda + causal_conv1d_cuda, sm_100a build) + reference op sequence, "
+               "kind": "reference CUDA ext (selective_scan_cuda + causal_conv1d_cuda, sm_90a build) + reference op sequence, "
                        "bf16 autocast, batch %d, %d^3 patch, same GPU" % (args.batch, args.patch)}
         del ref_step, params
         gc.collect()
@@ -342,10 +355,11 @@ def main_native(args):
     _lib.lib()   # fail loudly now if the native library is missing
 
     torch.manual_seed(0)
-    torch.backends.cudnn.benchmark = True
-    # the library convolutions are autotuned over ALL cuDNN plans (torch's default stops after 10): 100.6 -> 96.9 ms per step in
-    # slot r2d.  The setting is process-wide, so the vs_ref_cuda leg (same process, afterwards) gets the same treatment.
-    torch.backends.cudnn.benchmark_limit = int(os.environ.get("SMB_CUDNN_BENCH_LIMIT", "0"))
+    # The library convolutions run the plan cuDNN's heuristics pick, not an autotuned one: autotuning times the plans at start-up,
+    # picks differently from process to process, and with the plan the rounding of every convolution changes -- two runs of the
+    # same build then differ by ~1e-2 in the logits, and by the speed of whichever plans won.  The setting is process-wide, so the
+    # vs_ref_cuda leg (same process, afterwards) gets the same treatment.
+    torch.backends.cudnn.benchmark = False
     model = SegMamba(in_chans=4, out_chans=4, depths=[2, 2, 2, 2], feat_size=[48, 96, 192, 384]).to(dev)
     if args.channels_last:
         model = model.to(memory_format=torch.channels_last_3d)
@@ -367,6 +381,19 @@ def main_native(args):
             net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local_rank], gradient_as_bucket_view=True)
     opt_params = mw.optimizer_parameters() if mw is not None else list(model.parameters())
     opt = torch.optim.SGD(opt_params, lr=1e-2, weight_decay=3e-5, momentum=0.99, nesterov=True)             # 3_train.py:51-52
+    # Every timed step is the FIRST step from the seeded initial weights: the weights and the optimizer's momentum are inputs of
+    # a step as much as the patch is, and the backward accumulates with fp32 atomics, so weights carried from step to step
+    # differ from run to run in the last bits -- which bf16 activations amplify to ~1e-2 of the logits within one step.
+    # Restoring costs two multi-tensor kernels per step (measured inside the timed region like everything else).
+    state = list({id(p): p for p in list(model.parameters()) + list(opt_params)}.values())
+    state0 = [p.detach().clone() for p in state]
+
+    @torch.no_grad()
+    def restore_state():
+        torch._foreach_copy_(state, state0)
+        bufs = [b for st in opt.state.values() for b in st.values() if torch.is_tensor(b)]
+        if bufs:
+            torch._foreach_zero_(bufs)                             # a zero momentum buffer gives the first step's update
     B, P = args.batch, args.patch
     g = torch.Generator().manual_seed(42 + rank)                                                           # trainer.py:331
     x_host = torch.rand(B, 4, P, P, P, generator=g).pin_memory()
@@ -379,6 +406,8 @@ def main_native(args):
     amp_dtype = torch.float16 if args.amp == "fp16" else torch.bfloat16
     scaler = torch.amp.GradScaler() if args.amp == "fp16" else None                                        # trainer.py:67
 
+    last = {}                                                      # what the most recent step computed (--dump-outputs)
+
     def step(x, y):
         opt.zero_grad(set_to_none=True)
         if mw is not None:
@@ -386,6 +415,7 @@ def main_native(args):
         with torch.autocast("cuda", dtype=amp_dtype):
             logits = net(x.contiguous(memory_format=mf))
             loss = torch.nn.functional.cross_entropy(logits.float(), y)
+        last["logits"] = logits
         if scaler is not None:                                                                             # trainer.py:461-466
             scaler.scale(loss).backward()
             if mw is not None:
@@ -421,6 +451,7 @@ def main_native(args):
             return graphed(x, y)
 
     def e2e_step():
+        restore_state()
         xd = x_host.to(dev, non_blocking=True)
         yd = y_host.to(dev, non_blocking=True)
         loss = step(xd, yd)
@@ -468,14 +499,27 @@ def main_native(args):
     sampler = ClockSampler(local_rank)
     launches0 = _lib.launch_count()
     sampler.start()
+
+    def timed_step():
+        restore_state()
+        last["loss"] = step(x_dev, y_dev)
+
     if graphed is None:
         with _lib.profile() as prof:
-            total_ms = timed(lambda: step(x_dev, y_dev), args.steps)
+            total_ms = timed(timed_step, args.steps)
             durs = prof.durations()
     else:
-        total_ms = timed(lambda: step(x_dev, y_dev), args.steps)
+        total_ms = timed(timed_step, args.steps)
     clocks = sampler.stop()
     launches = _lib.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        # what a caller of the last timed step holds afterwards: its loss, its logits (an eager step; a replayed graph hands
+        # back the loss only) and the parameters after its update, through which its gradients show
+        with torch.no_grad():
+            out = {"loss": last["loss"].reshape(1), "params": torch.cat([p.reshape(-1).float() for p in opt_params])}
+            if "logits" in last and graphed is None:
+                out["logits"] = last["logits"]
+            dump_outputs(args.dump_outputs, out)
     if graphed is not None:
         launches = graph_launches * args.steps      # native kernel nodes replayed from the graph
         with _lib.profile() as prof:                # per-op timings need eager launches: taken right after the timed region
@@ -501,8 +545,8 @@ def main_native(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "data sheet, H100 SXM HBM3: 3350 GB/s (not a measured peak)"
 
     def roof(op, bytes_fn):
         metas = [m for (o, m) in durs if o == op]
@@ -513,23 +557,22 @@ def main_native(args):
         ms = sum(d) / len(d)
         by = bytes_fn(meta)
         ach = by / (ms * 1e-3) / 1e9
-        traffic = NCU_DRAM_BYTES.get((op,) + tuple(meta[:5]))
-        return {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": traffic,
-                "traffic_source": NCU_DRAM_SOURCE if traffic is not None else None,
+        return {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak, "traffic": None,
+                "traffic_source": None,
                 "kernel": f"smb_{op} (all passes) at batch={meta[0]} dim={meta[1]} L={meta[2]} N={meta[3]} elt={meta[4]}B",
                 "algorithmic_bytes": by, "avg_ms": ms, "launches_timed": len(d), "peak_source": peak_src}
 
     roof_fwd = roof("scan_fwd", scan_fwd_bytes)
     roof_bwd = roof("scan_bwd", scan_bwd_bytes)
     # The forward scan is co-bound by the MUFU pipe (DESIGN.md 3.1): one ex2 per (b, d, t, n) update in each of its two passes.
-    # Extra key, not part of the contract: ex2 throughput against 148 SMs x 16 lanes/clk at the SM clock sampled under load.
+    # Extra key, not part of the contract: ex2 throughput against 132 SMs x 16 lanes/clk at the SM clock sampled under load.
     roof_mufu = None
     try:
         if roof_fwd and clocks and clocks.get("sm_mhz"):
             b_, d_, l_, n_ = [int(v) for v in re.findall(r"batch=(\d+) dim=(\d+) L=(\d+) N=(\d+)", roof_fwd["kernel"])[0]]
             ex2 = 2.0 * b_ * d_ * l_ * n_
             ach = ex2 / (roof_fwd["avg_ms"] * 1e-3) / 1e12
-            peak = 148 * 16 * float(clocks["sm_mhz"]) * 1e6 / 1e12
+            peak = 132 * 16 * float(clocks["sm_mhz"]) * 1e6 / 1e12
             roof_mufu = {"bound": "mufu", "achieved": ach, "peak": peak, "unit": "Tex2/s", "frac": ach / peak,
                          "ex2_per_call": ex2, "kernel": roof_fwd["kernel"]}
     except Exception:
@@ -581,7 +624,7 @@ def main_native(args):
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": args.amp,
             "data": "synthetic",
             "config": {"workload": workload_name(args), "global_batch": world * B, "parallelism": f"dp{world}",
-                       "l2": "inputs larger than L2: one step touches > 10 GB of activations (126 MB L2)",
+                       "l2": "inputs larger than L2: one step touches > 10 GB of activations (50 MB L2)",
                        "channels_last_3d": (all(layout_seen.values()) if layout_seen else None), "cuda_graph": bool(args.cuda_graph), "bf16_params": bool(args.bf16_params)},
             "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
             "roofline": roofline,
@@ -638,7 +681,7 @@ def main_sliding_window(args):
         dist.barrier()
     _lib.lib()
     torch.manual_seed(0)
-    torch.backends.cudnn.benchmark = True
+    torch.backends.cudnn.benchmark = False                         # heuristic plans: the same arithmetic in every run (see main_native)
     model = SegMamba(in_chans=4, out_chans=4, depths=[2, 2, 2, 2], feat_size=[48, 96, 192, 384]).to(dev).eval()
     if world > 1:                                     # same weights everywhere (each rank seeded identically anyway)
         for p_ in model.parameters():
@@ -682,6 +725,8 @@ def main_sliding_window(args):
     e.record()
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"blended_logits": out})
     ms = torch.tensor([s.elapsed_time(e)], device=dev)
     if world > 1:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)

@@ -1,5 +1,5 @@
 /*
- * segmamba_b200.h -- C ABI of the B200-native SegMamba hot path (libsegmamba_b200.so).
+ * segmamba_b200.h -- C ABI of the H100-native (sm_90a) SegMamba hot path (libsegmamba_b200.so).
  *
  * Plain C: raw device pointers, sizes, element strides, a cudaStream_t passed as void*.  No torch
  * types.  Every entry point returns 0 on success or a negative SMB_E* code; smb_last_error() then
@@ -111,7 +111,7 @@ typedef struct smb_scan_bwd_args {
     int32_t delta_softplus;
     int32_t direction;
     int32_t low_memory;         /* 1: chunk-parallel recompute in registers, workspace of a few MB (the shim's default and
-                                      the faster path as measured on B200);
+                                      the default path);
                                    0: stash every recomputed state in the workspace (batch*L*dstate*dim elements) and
                                       sweep backwards once -- fewer instructions per update, more HBM traffic */
     const void *u, *delta, *z /* may be NULL */;
@@ -272,7 +272,7 @@ SMB_API int smb_layernorm_fwd(const smb_layernorm_args *args, void *cuda_stream)
 SMB_API int smb_layernorm_bwd(const smb_layernorm_bwd_args *args, void *cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Tensor-core GEMM (tcgen05.mma, accumulator in tensor memory, operands staged by TMA):
+ * Tensor-core GEMM (wgmma.mma_async, accumulator in registers, operands staged by TMA):
  *     D[M, N] = epilogue( A[M, K] . B[N, K]^T )        fp16 / bf16 operands, fp32 accumulation
  * a_major / b_major: SMB_MAJOR_K  -- the operand is stored (rows = M or N index, K contiguous), ld = row stride;
  *                    SMB_MAJOR_MN -- the operand is stored (rows = K index, M or N contiguous), ld = row stride.

@@ -1,7 +1,7 @@
-"""Generate golden vectors from the REFERENCE's own Python (run in the build container only).
+"""Generate golden vectors from the REFERENCE's own Python (needs the reference checkout).
 
 TEST INFRASTRUCTURE.  Imports /root/reference (read-only) and writes small fixtures under
-tests/golden/.  /root/reference does not exist on the GPU box, so nothing else may import this.
+tests/golden/.  Nothing else may import this.
 
 What is executed is the reference's code, unmodified:
   * selective_scan_ref          mamba/mamba_ssm/ops/selective_scan_interface.py:86-152

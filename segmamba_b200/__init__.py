@@ -1,4 +1,4 @@
-"""segmamba_b200 -- B200-native (sm_100a) implementation of the SegMamba hot path.
+"""segmamba_b200 -- H100-native (sm_90a) implementation of the SegMamba hot path.
 
 Public surface (mirrors the reference's, see INTEGRATION.md):
 

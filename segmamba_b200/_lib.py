@@ -129,7 +129,7 @@ _lock = threading.Lock()
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a with nvcc (cross-compiles without a GPU). Returns the .so path."""
+    """Compile the CUDA sources for sm_90a with nvcc (cross-compiles without a GPU). Returns the .so path."""
     cmd = ["make", "-C", CSRC, "-j8", "all"]
     if not verbose:
         cmd.insert(1, "-s")

@@ -15,7 +15,7 @@ namespace smb {
 static std::atomic<unsigned long long> g_launches{0};
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 #ifdef SMB_EMU
-// tcgen05 / tensor memory have no CPU emulation: the emulated library exports smb_gemm but every call fails loudly
+// wgmma / TMA have no CPU emulation: the emulated library exports smb_gemm but every call fails loudly
 cudaError_t gemm_tc_launch(GemmP, const void *, int64_t, const void *, int64_t, cudaStream_t, const char **) { return cudaErrorNotSupported; }
 int gemm_pick_bn(int) { return 0; }
 #endif
@@ -404,7 +404,7 @@ SMB_API int smb_gemm(const smb_gemm_args *a, void *cuda_stream) {
     p.split_k = a->split_k < 1 ? 1 : a->split_k;
     p.atomic = (p.split_k > 1 || a->accumulate) ? 1 : 0;
     p.bias = a->bias; p.D = a->D; p.ldd = a->ldd;
-    {   // measurement aid: SMB_GEMM_PROF = device address (decimal) of 8 uint64 counters that receive the per-role wait cycles
+    {   // measurement aid: SMB_GEMM_PROF = device address (decimal) of 16 uint64 counters that receive the per-role wait cycles
         const char *pe = getenv("SMB_GEMM_PROF");
         p.prof = pe ? reinterpret_cast<unsigned long long *>(strtoull(pe, nullptr, 10)) : nullptr;
     }

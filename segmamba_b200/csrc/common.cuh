@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a scan / conv kernels.
+// Shared device helpers for the sm_90a scan / conv kernels.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -42,29 +42,32 @@ __device__ __forceinline__ float ex2(float x) {
     return y;
 }
 #endif
-// ---- packed fp32x2 (Blackwell FFMA2 / FMUL2 / FADD2: two lanes of fp32 per issue slot) ----
+// ---- fp32 pairs: the kernels keep two states per float2; sm_90 has no packed fp32 arithmetic, so each op is two scalar ones ----
 __device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 ex2x2_mufu(float2 x) { return make_float2(ex2(x.x), ex2(x.y)); }
 // 2^x for x <= 0 on the FMA pipe (Cody-Waite split + degree-6 polynomial, rel. error ~2e-7, same class as MUFU.EX2):
-// lets a fraction of the decays move off the MUFU pipe (see SMB_POLY_MASK below for what that measured).
+// lets a fraction of the decays move off the MUFU pipe (see SMB_POLY_MASK below).
 __device__ __forceinline__ float2 ex2x2_poly(float2 x) {
     x.x = fmaxf(x.x, -126.f);
     x.y = fmaxf(x.y, -126.f);
-    const float2 t = __fadd2_rn(x, f2(12582912.f, 12582912.f));          // round to nearest integer in the low mantissa bits
-    const float2 n = __fadd2_rn(t, f2(-12582912.f, -12582912.f));
-    const float2 f = __ffma2_rn(n, f2(-1.f, -1.f), x);                    // f in [-0.5, 0.5]
+    const float2 t = fadd2(x, f2(12582912.f, 12582912.f));          // round to nearest integer in the low mantissa bits
+    const float2 n = fadd2(t, f2(-12582912.f, -12582912.f));
+    const float2 f = ffma2(n, f2(-1.f, -1.f), x);                    // f in [-0.5, 0.5]
     float2 p = f2(1.535336188319500e-4f, 1.535336188319500e-4f);
-    p = __ffma2_rn(p, f, f2(1.339887440266574e-3f, 1.339887440266574e-3f));
-    p = __ffma2_rn(p, f, f2(9.618437357674640e-3f, 9.618437357674640e-3f));
-    p = __ffma2_rn(p, f, f2(5.550332471162809e-2f, 5.550332471162809e-2f));
-    p = __ffma2_rn(p, f, f2(2.402264791363012e-1f, 2.402264791363012e-1f));
-    p = __ffma2_rn(p, f, f2(6.931472028550421e-1f, 6.931472028550421e-1f));
-    p = __ffma2_rn(p, f, f2(1.f, 1.f));
+    p = ffma2(p, f, f2(1.339887440266574e-3f, 1.339887440266574e-3f));
+    p = ffma2(p, f, f2(9.618437357674640e-3f, 9.618437357674640e-3f));
+    p = ffma2(p, f, f2(5.550332471162809e-2f, 5.550332471162809e-2f));
+    p = ffma2(p, f, f2(2.402264791363012e-1f, 2.402264791363012e-1f));
+    p = ffma2(p, f, f2(6.931472028550421e-1f, 6.931472028550421e-1f));
+    p = ffma2(p, f, f2(1.f, 1.f));
     return make_float2(__int_as_float(__float_as_int(p.x) + (__float_as_int(t.x) << 23)),
                        __int_as_float(__float_as_int(p.y) + (__float_as_int(t.y) << 23)));
 }
-// which state pairs take the polynomial path (bit m = pair m).  Measured on B200 (stage 0, bf16): 0x00 0.658 ms, 0x11 0.689 ms,
-// 0x55 0.793 ms -- the kernels are issue-bound, not MUFU-bound, so the default keeps every decay on the MUFU.
+// which state pairs take the polynomial path (bit m = pair m).  The default keeps every decay on the MUFU; other masks have not
+// been measured on H100.
 #ifndef SMB_POLY_MASK
 #define SMB_POLY_MASK 0x00
 #endif

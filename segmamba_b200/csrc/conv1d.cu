@@ -1,4 +1,4 @@
-// Depthwise causal conv1d (+SiLU) forward / backward for sm_100a, and the inter-slice sequence permutation.
+// Depthwise causal conv1d (+SiLU) forward / backward for sm_90a, and the inter-slice sequence permutation.
 //
 // Restates causal_conv1d_fwd_kernel / causal_conv1d_bwd_kernel (causal-conv1d/csrc/causal_conv1d_fwd.cu:39-130,
 // causal_conv1d_bwd.cu:46-240).  The reference runs one CTA per (batch, channel) that walks L serially in

@@ -1,7 +1,6 @@
 // Depthwise causal conv1d forward / backward with 16 scan positions per thread for 16-bit activations
 // (opt-in: SMB_CONV_V2=1).  Same arithmetic as conv1d.cu.  Why: with 8 positions per thread a bf16 / fp16 thread moves only
-// 16 bytes each way and the kernel reaches 47 % of the HBM peak where the fp32 instantiation (32 bytes per thread) reaches
-// 93 % (profiles/r1_microbench_final.json); 16 positions give the 16-bit types the same bytes in flight per thread.
+// 16 bytes each way, half of what the fp32 instantiation (32 bytes per thread) keeps in flight; 16 positions give the 16-bit types the same bytes in flight per thread.
 #include "conv_internal.h"
 
 #include <cstdint>
@@ -182,8 +181,8 @@ static cudaError_t conv2_launch_t(const ConvP &p, bool bwd, cudaStream_t st) {
 
 // ---------------------------------------------------------------------------------------------
 // inter-slice permutation for 16-bit activations with 4-byte accesses (opt-in: SMB_PERMUTE_V2=1).
-// The default kernel (conv1d.cu) moves one 2-byte element per thread and access: a warp touches 64 bytes per row segment and
-// reaches 2.9 TB/s on the stage-0 tensor (profiles/r1_op_breakdown_final.txt).  Here a CTA transposes a 64 x 64 tile held as
+// The default kernel (conv1d.cu) moves one 2-byte element per thread and access: a warp touches 64 bytes per row segment.
+// Here a CTA transposes a 64 x 64 tile held as
 // 64 x 32 words: every global access is a 128-byte row segment of 32 element pairs; the pair that leaves along the
 // destination row is assembled from the same half of two vertically adjacent words (one PRMT).
 // Requires even n_src_rows / n_src_cols and 4-byte aligned rows; the dispatcher falls back to the default kernel otherwise.

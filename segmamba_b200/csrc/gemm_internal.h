@@ -17,11 +17,11 @@ struct GemmP {
     int epilogue;           // GEMM_EPI_*
     int atomic;             // fp32 output only: atomicAdd into D (split-K partial products; D zero-initialised by the caller)
     int split_k;            // number of K slices handled by different CTAs (requires atomic when > 1)
-    int BN, stages, tmem_cols;   // filled by the launcher (BN may be preset: multiple of 16, <= 256)
+    int BN, stages;         // filled by the launcher (BN may be preset: one of the tile widths gemm_pick_bn returns)
     const float *bias;
     void *D;
     int64_t ldd;            // elements
-    unsigned long long *prof;   // optional 8 device counters: cycles in barrier waits per role (gemm_tc.cu), else nullptr
+    unsigned long long *prof;   // optional 16 device counters: cycles in barrier waits per role (gemm_tc.cu), else nullptr
 };
 
 int gemm_pick_bn(int N);

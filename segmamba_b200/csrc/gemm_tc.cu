@@ -1,5 +1,5 @@
-// Tensor-core GEMM for the pointwise contractions of the SegMamba hot path (sm_100a: TMA -> shared memory -> tcgen05.mma with
-// the accumulator in tensor memory -> tcgen05.ld epilogue).
+// Tensor-core GEMM for the pointwise contractions of the SegMamba hot path (sm_90a: TMA -> shared memory -> wgmma.mma_async with
+// the accumulator in registers -> staged, coalesced epilogue).
 //
 //     D[M, N] (+)= epilogue( A[M, K] . B[N, K]^T )          16-bit operands, fp32 accumulation
 //
@@ -9,18 +9,20 @@
 // backward products (data gradient: the same kernel on the transposed weight view; weight gradient: contraction over the token
 // axis, both operands MN-major, split over CTAs along K with fp32 atomics).
 //
-// Structure (one persistent CTA per SM, 320 threads, warp-specialised):
-//   warp 0      TMA producer: cp.async.bulk.tensor 2-D boxes of A (128 x 64) and B (BN x 64) per 64-wide K block into a
-//               ring of shared-memory stages (CU_TENSOR_MAP_SWIZZLE_128B), completion on the stage's `full` mbarrier
-//   warp 1      allocates tensor memory; one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M = 128, N = BN, K = 16)
-//               four per K block, releases the stage with tcgen05.commit -> `empty`, and after the last K block commits to
-//               the accumulator's `tmem_full` barrier.  Two accumulator buffers (2 x BN columns) overlap the epilogue of
-//               tile i with the main loop of tile i + 1.
-//   warps 2..5  epilogue: tcgen05.ld (32 lanes x 16 columns per instruction) -> bias / GELU -> convert -> padded staging tile
-//               in shared memory -> coalesced 16-byte global stores (or fp32 atomics for split-K) by the same 128 threads.
+// Structure (one persistent CTA per SM, 384 threads = three warpgroups, warp-specialised):
+//   warpgroup 0     TMA producer (one thread; the warpgroup gives its registers up with setmaxnreg): cp.async.bulk.tensor 2-D
+//                   boxes of A (128 x 64) and B (BN x 64) per 64-wide K block into a ring of shared-memory stages
+//                   (CU_TENSOR_MAP_SWIZZLE_128B), completion on the stage's `full` mbarrier
+//   warpgroups 1,2  consumers: each owns 64 rows of the 128 x BN tile.  Per K block four wgmma.mma_async k16 steps per 64-column
+//                   chunk of the tile (m64n64k16, or n16 / n32 / n48 for the last chunk), one commit group per K block with one
+//                   group in flight; a stage is released to the producer (`empty` mbarrier, one arrival per warp) when the
+//                   group that read it has completed.  Epilogue by the same warps: bias / GELU -> convert -> warp-private
+//                   padded staging tile in shared memory -> coalesced 16-byte global stores (or fp32 atomics for split-K),
+//                   while the producer already fills the ring for the next tile.
+// BN is a template parameter (the wgmma shape is part of the instruction): 16, 32, 48, 64, 96, 128, 192 or 256.
 // Either operand may be K-major (rows = M or N index, K contiguous) or MN-major (rows = K index, M or N contiguous); the
-// shared-memory matrix descriptors and the instruction descriptor carry the difference, the TMA boxes stay (64 elements = 128
-// bytes) x rows.  Out-of-range rows / columns of a box are zero-filled by the TMA unit, so ragged M, N and K need no separate
+// shared-memory matrix descriptors and the instruction's transpose bits carry the difference, the TMA boxes stay (64 elements =
+// 128 bytes) x rows.  Out-of-range rows / columns of a box are zero-filled by the TMA unit, so ragged M, N and K need no separate
 // path on the load side; the store side bounds every access.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -37,12 +39,14 @@ void count_launch();
 
 namespace {
 
-constexpr int kBM = 128;            // UMMA M (one CTA, cta_group::1): accumulator row i lives in tensor-memory lane i
+constexpr int kBM = 128;            // two consumer warpgroups x wgmma M = 64
 constexpr int kBK = 64;             // K block: 64 sixteen-bit elements = one 128-byte swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kThreads = 320;          // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quadrant)
-constexpr int kEpiWarps = 8;
+constexpr int kMmaK = 16;
+constexpr int kThreads = 384;       // warpgroup 0 TMA, warpgroups 1..2 wgmma + epilogue
+constexpr int kConsumerWarps = 8;
 constexpr int kMaxStages = 6;
+constexpr int kPitch = 144;         // staging row pitch: 128 + 16 bytes -> conflict-free 16-byte reads
+constexpr int kStagingBytes = kConsumerWarps * 16 * kPitch;
 
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return static_cast<unsigned>(__cvta_generic_to_shared(p)); }
 
@@ -87,52 +91,52 @@ __device__ __forceinline__ void tma_load_2d(void *smem, const CUtensorMap *m, in
                  "l"(m), "r"(c0), "r"(c1), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma(unsigned d_tmem, uint64_t a_desc, uint64_t b_desc, unsigned idesc, unsigned accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tc_ld16(unsigned taddr, float (&v)[16]) {
-    unsigned r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        "tcgen05.wait::ld.sync.aligned;\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+template <typename T> constexpr bool kIsBf16 = false;
+template <> constexpr bool kIsBf16<__nv_bfloat16> = true;
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending> __device__ __forceinline__ void wg_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
 
-__device__ __forceinline__ void tc_ld32(unsigned taddr, unsigned (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-          "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]),
-          "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+// D (64 x N fp32, in registers) = A . B (+ D when scale_d != 0), both operands through shared-memory descriptors; TA / TB = 1
+// marks an MN-major operand.  The accumulator fragment of a thread: d[4 j + {0, 1}] = row (lane / 4) of its warp's 16 rows,
+// columns 8 j + 2 (lane % 4) + {0, 1}; d[4 j + {2, 3}] = row (lane / 4) + 8, same columns.
+#define SMB_ACC8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+#define SMB_D8 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define SMB_D16 SMB_D8 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define SMB_D24 SMB_D16 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define SMB_D32 SMB_D24 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define SMB_WGMMA(SHAPE, TYPE, DREGS, OA, OB, OS, OTA, OTB, ...)                                                             \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" OS ", 0;\n"                                                             \
+                 "wgmma.mma_async.sync.aligned." SHAPE ".f32." TYPE "." TYPE " {" DREGS "}, %" OA ", %" OB ", p, 1, 1, %" OTA \
+                 ", %" OTB ";\n}\n"                                                                                           \
+                 : __VA_ARGS__                                                                                                \
+                 : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB))
+#define SMB_WGMMA_N(TYPE)                                                                                                     \
+    if constexpr (N == 64) SMB_WGMMA("m64n64k16", TYPE, SMB_D32, "32", "33", "34", "35", "36", SMB_ACC8(0), SMB_ACC8(8), SMB_ACC8(16), SMB_ACC8(24)); \
+    else if constexpr (N == 48) SMB_WGMMA("m64n48k16", TYPE, SMB_D24, "24", "25", "26", "27", "28", SMB_ACC8(0), SMB_ACC8(8), SMB_ACC8(16));        \
+    else if constexpr (N == 32) SMB_WGMMA("m64n32k16", TYPE, SMB_D16, "16", "17", "18", "19", "20", SMB_ACC8(0), SMB_ACC8(8));                     \
+    else SMB_WGMMA("m64n16k16", TYPE, SMB_D8, "8", "9", "10", "11", "12", SMB_ACC8(0))
+template <typename TIn, int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_k16(float (&d)[32], uint64_t da, uint64_t db, unsigned scale_d) {
+    static_assert(N == 16 || N == 32 || N == 48 || N == 64, "chunk width");
+    if constexpr (kIsBf16<TIn>) { SMB_WGMMA_N("bf16"); } else { SMB_WGMMA_N("f16"); }
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+#undef SMB_WGMMA_N
+#undef SMB_WGMMA
+#undef SMB_D32
+#undef SMB_D24
+#undef SMB_D16
+#undef SMB_D8
+#undef SMB_ACC8
 __device__ __forceinline__ void red_add_v4f(float *a, float x, float y, float z, float w) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(a), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
 }
 
-// shared-memory matrix descriptor, 128-byte swizzle (cute::UMMA::SmemDescriptor: start >> 4 at [0,14), leading byte offset >> 4
-// at [16,30), stride byte offset >> 4 at [32,46), version 1 at [46,48), layout type SWIZZLE_128B = 2 at [61,64)).
+// shared-memory matrix descriptor, 128-byte swizzle (start >> 4 at [0,14), leading byte offset >> 4 at [16,30), stride byte
+// offset >> 4 at [32,46), swizzle mode 128B = 1 at [62,64)).
 //   K-major  tile = rows x 128 B : 8-row groups are 1024 B apart (SBO); the leading offset is unused inside one swizzle row.
 //   MN-major tile = 64 K-rows x 128 B per 64 MN elements: 8-K-row groups 1024 B apart (SBO), next 64 MN elements one tile on (LBO).
 __device__ __forceinline__ uint64_t make_desc(unsigned smem_addr, unsigned lbo_bytes, unsigned sbo_bytes) {
@@ -140,8 +144,7 @@ __device__ __forceinline__ uint64_t make_desc(unsigned smem_addr, unsigned lbo_b
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
 
@@ -159,17 +162,6 @@ template <> __device__ __forceinline__ unsigned pack2<__half>(float a, float b) 
     return *reinterpret_cast<unsigned *>(&h);
 }
 
-// packed 16-bit pair `old` + (a, b), rounded once
-template <typename T> __device__ __forceinline__ unsigned add2(unsigned old, float a, float b);
-template <> __device__ __forceinline__ unsigned add2<__nv_bfloat16>(unsigned old, float a, float b) {
-    const __nv_bfloat162 o = *reinterpret_cast<const __nv_bfloat162 *>(&old);
-    return pack2<__nv_bfloat16>(__low2float(o) + a, __high2float(o) + b);
-}
-template <> __device__ __forceinline__ unsigned add2<__half>(unsigned old, float a, float b) {
-    const __half2 o = *reinterpret_cast<const __half2 *>(&old);
-    return pack2<__half>(__low2float(o) + a, __high2float(o) + b);
-}
-
 template <typename T> __device__ __forceinline__ unsigned sum2(unsigned a, unsigned b);
 template <> __device__ __forceinline__ unsigned sum2<__nv_bfloat16>(unsigned a, unsigned b) {
     const __nv_bfloat162 x = *reinterpret_cast<const __nv_bfloat162 *>(&a), y = *reinterpret_cast<const __nv_bfloat162 *>(&b);
@@ -181,43 +173,68 @@ template <> __device__ __forceinline__ unsigned sum2<__half>(unsigned a, unsigne
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
-// TOut: __nv_bfloat16 / __half (store) or float (store, or atomic accumulate when p.atomic)
+// main loop of one tile for one consumer warpgroup: acc (64 x BN) = A[64 rows] . B^T over the K blocks [kb0, kb1)
 // ---------------------------------------------------------------------------------------------------------------------------
-template <typename TOut>
+template <typename TIn, int BN, int TA, int TB>
+__device__ __forceinline__ void consume_tile(float (&acc)[(BN + 63) / 64][32], const GemmP &p, unsigned stage0, int stage_bytes,
+                                             uint64_t *full, uint64_t *empty, int kb0, int kb1, unsigned &it, int cw, int lane) {
+    constexpr int kChunks = (BN + 63) / 64, kLast = BN - 64 * (kChunks - 1);
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % p.stages;
+        mbar_wait_prof(&full[s], (it / p.stages) & 1, (p.prof && cw == 0 && threadIdx.x % 128 == 0) ? p.prof + 2 : nullptr);
+        const unsigned sa = stage0 + (unsigned)(s * stage_bytes) + (unsigned)(cw * 8192), sb = stage0 + (unsigned)(s * stage_bytes) + kBM * 128;
+        wg_fence();
+        // a K tail needs no shorter loop: the TMA unit zero-filled the K positions past p.K in both operands
+#pragma unroll
+        for (int k = 0; k < kBK / kMmaK; ++k) {
+            const uint64_t da = TA ? make_desc(sa + k * (kMmaK * 128), 8192, 1024) : make_desc(sa + k * (kMmaK * 2), 16, 1024);
+            const unsigned acc_on = (kb > kb0 || k > 0) ? 1u : 0u;
+#pragma unroll
+            for (int c = 0; c < kChunks; ++c) {
+                const uint64_t db = TB ? make_desc(sb + c * 8192 + k * (kMmaK * 128), 8192, 1024)
+                                       : make_desc(sb + c * 8192 + k * (kMmaK * 2), 16, 1024);
+                if (c + 1 < kChunks) wgmma_k16<TIn, 64, TA, TB>(acc[c], da, db, acc_on);
+                else wgmma_k16<TIn, kLast, TA, TB>(acc[c], da, db, acc_on);
+            }
+        }
+        wg_commit();
+        if (prev >= 0) {                                  // the group of the previous K block has completed: release its stage
+            wg_wait<1>();
+            if (lane == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = s;
+    }
+    wg_wait<0>();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// TIn: __nv_bfloat16 / __half operands.  TOut: TIn (store) or float (store, or atomic accumulate when p.atomic)
+// ---------------------------------------------------------------------------------------------------------------------------
+template <typename TIn, typename TOut, int BN>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA,
                                                               const __grid_constant__ CUtensorMap tmB, const GemmP p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    const int BN = p.BN;
-    const int a_tile = kBM * 128;                       // bytes per stage
-    const int b_rows = p.b_mn ? ((BN + 63) / 64) * 64 : BN;
-    const int b_tile = p.b_mn ? ((BN + 63) / 64) * 8192 : BN * 128;
+    constexpr int kChunks = (BN + 63) / 64;
+    constexpr int a_tile = kBM * 128;                       // bytes per stage
+    const int b_tile = p.b_mn ? kChunks * 8192 : BN * 128;
     const int stage_bytes = a_tile + ((b_tile + 1023) & ~1023);
     uint8_t *stage0 = smem;
-    uint8_t *staging = smem + (size_t)p.stages * stage_bytes;                 // 8 warps x 32 rows x 144 bytes
-    uint64_t *bars = reinterpret_cast<uint64_t *>(staging + kEpiWarps * 32 * 144);
-    uint64_t *full = bars, *empty = bars + kMaxStages, *tfull = bars + 2 * kMaxStages, *tempty = bars + 2 * kMaxStages + 2;
-    unsigned *tmem_slot = reinterpret_cast<unsigned *>(bars + 2 * kMaxStages + 4);
-    (void)b_rows;
+    uint8_t *staging = smem + (size_t)p.stages * stage_bytes;                 // 8 warps x 16 rows x 144 bytes
+    uint64_t *bars = reinterpret_cast<uint64_t *>(staging + kStagingBytes);
+    uint64_t *full = bars, *empty = bars + kMaxStages;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], kEpiWarps); }
+        for (int s = 0; s < p.stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(p.tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const unsigned tmem_base = *tmem_slot;
     const long long t_start = clock64();
 
     const int m_tiles = (p.M + kBM - 1) / kBM;
@@ -226,8 +243,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int kb_per = (kb_total + p.split_k - 1) / p.split_k;
     const int n_work = m_tiles * n_tiles * p.split_k;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
             unsigned it = 0;
             for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
                 const int sp = t % p.split_k, nb = (t / p.split_k) % n_tiles, mb = t / (p.split_k * n_tiles);
@@ -247,182 +265,132 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     if (!p.b_mn) {
                         tma_load_2d(sb, &tmB, kb * kBK, nb * BN, &full[s]);
                     } else {
-                        for (int c = 0; c * 64 < BN; ++c) tma_load_2d(sb + c * 8192, &tmB, nb * BN + c * 64, kb * kBK, &full[s]);
+                        for (int c = 0; c < kChunks; ++c) tma_load_2d(sb + c * 8192, &tmB, nb * BN + c * 64, kb * kBK, &full[s]);
                     }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 at [4,6), a / b format (F16 0, BF16 1) at
-            // [7,10) / [10,13), a / b major (0 K, 1 MN) at bits 15 / 16, N >> 3 at [17,23), M >> 4 at [24,29)
-            const unsigned fmt = p.dtype == 2 ? 1u : 0u;
-            const unsigned idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((unsigned)p.a_mn << 15) | ((unsigned)p.b_mn << 16) |
-                                   ((unsigned)(BN >> 3) << 17) | ((unsigned)(kBM >> 4) << 24);
-            unsigned it = 0, tc = 0;
-            for (int t = blockIdx.x; t < n_work; t += gridDim.x, ++tc) {
-                const int sp = t % p.split_k;
-                const int kb0 = sp * kb_per, kb1 = min(kb_total, kb0 + kb_per);
-                const int as = tc & 1;
-                mbar_wait_prof(&tempty[as], ((tc >> 1) & 1) ^ 1, p.prof ? p.prof + 1 : nullptr);
-                tc_fence_after();
-                const unsigned d_tmem = tmem_base + (unsigned)(as * BN);
-                for (int kb = kb0; kb < kb1; ++kb, ++it) {
-                    const int s = it % p.stages;
-                    mbar_wait_prof(&full[s], (it / p.stages) & 1, p.prof ? p.prof + 2 : nullptr);
-                    tc_fence_after();
-                    const unsigned sa = smem_u32(stage0 + (size_t)s * stage_bytes), sb = sa + a_tile;
-                    const int k_left = p.K - kb * kBK;
-                    const int nk = k_left >= kBK ? kBK / kUmmaK : (k_left + kUmmaK - 1) / kUmmaK;
-                    for (int k = 0; k < nk; ++k) {
-                        const uint64_t da = p.a_mn ? make_desc(sa + k * (kUmmaK * 128), 8192, 1024) : make_desc(sa + k * (kUmmaK * 2), 16, 1024);
-                        const uint64_t db = p.b_mn ? make_desc(sb + k * (kUmmaK * 128), 8192, 1024) : make_desc(sb + k * (kUmmaK * 2), 16, 1024);
-                        tc_mma(d_tmem, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-                    }
-                    tc_commit(&empty[s]);                 // the stage may be refilled once these MMAs have read it
-                }
-                tc_commit(&tfull[as]);                    // accumulator complete
             }
         }
     } else {
-        // ------------------------------- epilogue warps (2..5): TMEM lane quadrant = warp % 4 -------------------------------
-        // A thread drains one accumulator row (its TMEM lane), 32 columns per tcgen05.ld with the next load in flight, and parks
-        // the converted values in a warp-private staging tile of 32 rows x 128 bytes; the warp then writes the tile out with 8
-        // lanes per row, i.e. one full 128-byte line per row and four lines per store instruction.  (Storing each thread's own row
-        // straight from registers costs one LSU transaction per 16 bytes: measured 3.2 us per 128 x 256 tile, four times the
-        // HBM time of the tile.)  No CTA-level barrier: the tile is private to the warp.
-        const int q = warp & 3;                          // TMEM lanes 32 q .. 32 q + 31 (a warp may only touch its own quadrant)
-        const int half = (warp - 2) >> 2;                // two warps share a quadrant: each drains half of the column groups
-        unsigned tc = 0;
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        // ------------------------------------ consumer warpgroups: rows 64 cw .. 64 cw + 63 ------------------------------------
+        // After the main loop a warp holds 16 rows of the tile.  It parks kGC converted columns at a time in its private staging
+        // tile of 16 rows x 128 bytes and writes the tile out with 8 lanes per row, i.e. one full 128-byte line per row and four
+        // lines per store instruction (the fragment's own layout would store 4- or 8-byte pieces).  No CTA-level barrier: the
+        // tile is private to the warp.
+        const int cw = (warp >> 2) - 1, wq = warp & 3;
+        const int r0 = lane >> 2, q = lane & 3;
         TOut *const D = reinterpret_cast<TOut *>(p.D);
-        constexpr int kPitch = 144;                      // staging row pitch: 128 + 16 bytes -> conflict-free 16-byte accesses
         constexpr int kGC = 128 / (int)sizeof(TOut);     // columns per staged group: 64 (16-bit) or 32 (fp32)
         constexpr int kVec = 16 / (int)sizeof(TOut);
-        uint8_t *stg = staging + (size_t)(warp - 2) * (32 * kPitch);
-        for (int t = blockIdx.x; t < n_work; t += gridDim.x, ++tc) {
+        uint8_t *stg = staging + (size_t)(warp - 4) * (16 * kPitch);
+        const unsigned stage0_addr = smem_u32(stage0);
+        float acc[kChunks][32];
+        unsigned it = 0;
+        for (int t = blockIdx.x; t < n_work; t += gridDim.x) {
             const int nb = (t / p.split_k) % n_tiles, mb = t / (p.split_k * n_tiles);
             const int sp = t % p.split_k;
-            const int as = tc & 1;
-            mbar_wait_prof(&tfull[as], (tc >> 1) & 1, (p.prof && lane == 0 && half == 0) ? p.prof + 3 + q : nullptr);
-            tc_fence_after();
+            const int kb0 = sp * kb_per, kb1 = min(kb_total, kb0 + kb_per);
+            switch (p.a_mn * 2 + p.b_mn) {
+                case 0: consume_tile<TIn, BN, 0, 0>(acc, p, stage0_addr, stage_bytes, full, empty, kb0, kb1, it, cw, lane); break;
+                case 1: consume_tile<TIn, BN, 0, 1>(acc, p, stage0_addr, stage_bytes, full, empty, kb0, kb1, it, cw, lane); break;
+                case 2: consume_tile<TIn, BN, 1, 0>(acc, p, stage0_addr, stage_bytes, full, empty, kb0, kb1, it, cw, lane); break;
+                default: consume_tile<TIn, BN, 1, 1>(acc, p, stage0_addr, stage_bytes, full, empty, kb0, kb1, it, cw, lane); break;
+            }
             const long long t_tile0 = p.prof ? clock64() : 0;
-            const unsigned taddr = tmem_base + ((unsigned)(q * 32) << 16) + (unsigned)(as * BN);
             const int n0 = nb * BN;
-            const int m0 = mb * kBM + q * 32;             // first row of this warp
+            const int m0 = mb * kBM + cw * 64 + wq * 16;   // first row of this warp
             const int n_valid = min(BN, p.N - n0);
-            const float bias_m = (p.epilogue == GEMM_EPI_BIAS_M && p.bias && m0 + lane < p.M && sp == 0) ? p.bias[m0 + lane] : 0.f;
-            // column groups of this warp: [g_begin, g_end), the first / second half of the tile's groups
-            const int n_groups = (n_valid + kGC - 1) / kGC;
-            const int g_begin = half ? ((n_groups + 1) / 2) * kGC : 0;
-            const int g_end = half ? n_valid : min(n_valid, ((n_groups + 1) / 2) * kGC);
-            if (m0 < p.M && g_begin < g_end) {            // whole-warp condition: tcgen05.ld is .sync.aligned
-                unsigned cur[32];
-                tc_ld32(taddr + (unsigned)g_begin, cur);
-                for (int g0 = g_begin; g0 < g_end; g0 += kGC) {
+            const bool bias_m_on = p.epilogue == GEMM_EPI_BIAS_M && p.bias && sp == 0;
+            const float bias_m0 = (bias_m_on && m0 + r0 < p.M) ? p.bias[m0 + r0] : 0.f;
+            const float bias_m1 = (bias_m_on && m0 + r0 + 8 < p.M) ? p.bias[m0 + r0 + 8] : 0.f;
+            if (m0 < p.M) {
 #pragma unroll
-                    for (int h = 0; h < kGC / 32; ++h) {
-                        const int c0 = g0 + 32 * h;
-                        if (c0 < g_end) {
-                            const long long tq0 = p.prof ? clock64() : 0;
-                            tc_wait_ld();
-                            const long long tq1 = p.prof ? clock64() : 0;
-                            if (p.prof && warp == 2 && lane == 0) atomicAdd(p.prof + 8, (unsigned long long)(tq1 - tq0));
-                            float v[32];
+                for (int g0 = 0; g0 < BN; g0 += kGC) {
+                    if (g0 < n_valid) {
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(cur[i]);
-                            // the next 32 columns load into `cur` while `v` is converted and staged (v is live across the load, so
-                            // the two never share registers; `cur` is not read again before the next wait)
-                            if (c0 + 32 < g_end) tc_ld32(taddr + (unsigned)(c0 + 32), cur);
-                            if (p.epilogue == GEMM_EPI_BIAS_N || p.epilogue == GEMM_EPI_BIAS_N_GELU) {
-                                if (p.bias && sp == 0) {
+                        for (int jj = 0; jj < kGC / 8; ++jj) {
+                            const int j = g0 / 8 + jj;                    // 8-column block of the tile
+                            if (8 * j < BN) {
+                                const float *a4 = &acc[j / 8][4 * (j % 8)];
+                                float v[4] = {a4[0], a4[1], a4[2], a4[3]};
+                                const int col = 8 * j + 2 * q;
+                                if (p.epilogue == GEMM_EPI_BIAS_N || p.epilogue == GEMM_EPI_BIAS_N_GELU) {
+                                    if (p.bias && sp == 0) {
+                                        const float b0 = (n0 + col < p.N) ? __ldg(p.bias + n0 + col) : 0.f;
+                                        const float b1 = (n0 + col + 1 < p.N) ? __ldg(p.bias + n0 + col + 1) : 0.f;
+                                        v[0] += b0; v[1] += b1; v[2] += b0; v[3] += b1;
+                                    }
+                                    if (p.epilogue == GEMM_EPI_BIAS_N_GELU) {
 #pragma unroll
-                                    for (int i = 0; i < 32; ++i) v[i] += (n0 + c0 + i < p.N) ? __ldg(p.bias + n0 + c0 + i) : 0.f;
+                                        for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
+                                    }
+                                } else if (p.epilogue == GEMM_EPI_BIAS_M) {
+                                    v[0] += bias_m0; v[1] += bias_m0; v[2] += bias_m1; v[3] += bias_m1;
                                 }
-                                if (p.epilogue == GEMM_EPI_BIAS_N_GELU) {
-#pragma unroll
-                                    for (int i = 0; i < 32; ++i) v[i] = gelu_erf(v[i]);
+                                uint8_t *s0 = stg + r0 * kPitch + (8 * jj + 2 * q) * (int)sizeof(TOut), *s1 = s0 + 8 * kPitch;
+                                if constexpr (sizeof(TOut) == 4) {
+                                    *reinterpret_cast<float2 *>(s0) = make_float2(v[0], v[1]);
+                                    *reinterpret_cast<float2 *>(s1) = make_float2(v[2], v[3]);
+                                } else {
+                                    *reinterpret_cast<unsigned *>(s0) = pack2<TOut>(v[0], v[1]);
+                                    *reinterpret_cast<unsigned *>(s1) = pack2<TOut>(v[2], v[3]);
                                 }
-                            } else if (p.epilogue == GEMM_EPI_BIAS_M) {
-#pragma unroll
-                                for (int i = 0; i < 32; ++i) v[i] += bias_m;
-                            }
-                            uint8_t *srow = stg + lane * kPitch + h * 64;
-                            if constexpr (sizeof(TOut) == 4) {
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) *reinterpret_cast<F4 *>(srow + 16 * i) = F4{v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]};
-                            } else {
-#pragma unroll
-                                for (int i = 0; i < 4; ++i)
-                                    *reinterpret_cast<uint4 *>(srow + 16 * i) =
-                                        make_uint4(pack2<TOut>(v[8 * i], v[8 * i + 1]), pack2<TOut>(v[8 * i + 2], v[8 * i + 3]),
-                                                   pack2<TOut>(v[8 * i + 4], v[8 * i + 5]), pack2<TOut>(v[8 * i + 6], v[8 * i + 7]));
                             }
                         }
-                    }
-                    __syncwarp();
-                    const long long tq2 = p.prof ? clock64() : 0;
-                    // ---- write the group out: lane -> (row = 4 it + lane / 8, 16-byte piece = lane % 8) ----
+                        __syncwarp();
+                        // ---- write the group out: lane -> (row = 4 i4 + lane / 8, 16-byte piece = lane % 8) ----
 #pragma unroll
-                    for (int it = 0; it < 8; ++it) {
-                        const int r = 4 * it + (lane >> 3), pc = lane & 7;
-                        const int col = g0 + pc * kVec, m = m0 + r;
-                        if (m < p.M && col < n_valid) {
-                            const uint8_t *src = stg + r * kPitch + pc * 16;
-                            TOut *dst = D + (int64_t)m * p.ldd + n0 + col;
-                            const bool full = (col + kVec <= n_valid) && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
-                            if constexpr (sizeof(TOut) == 4) {
-                                const F4 sv = *reinterpret_cast<const F4 *>(src);
-                                float *fd = reinterpret_cast<float *>(dst);
-                                if (full) {
-                                    if (p.atomic) red_add_v4f(fd, sv.x, sv.y, sv.z, sv.w);
-                                    else *reinterpret_cast<F4 *>(fd) = sv;
-                                } else {
-                                    const float e4[4] = {sv.x, sv.y, sv.z, sv.w};
+                        for (int i4 = 0; i4 < 4; ++i4) {
+                            const int r = 4 * i4 + (lane >> 3), pc = lane & 7;
+                            const int col = g0 + pc * kVec, m = m0 + r;
+                            if (m < p.M && col < n_valid) {
+                                const uint8_t *src = stg + r * kPitch + pc * 16;
+                                TOut *dst = D + (int64_t)m * p.ldd + n0 + col;
+                                const bool full16 = (col + kVec <= n_valid) && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+                                if constexpr (sizeof(TOut) == 4) {
+                                    const F4 sv = *reinterpret_cast<const F4 *>(src);
+                                    float *fd = reinterpret_cast<float *>(dst);
+                                    if (full16) {
+                                        if (p.atomic) red_add_v4f(fd, sv.x, sv.y, sv.z, sv.w);
+                                        else *reinterpret_cast<F4 *>(fd) = sv;
+                                    } else {
+                                        const float e4[4] = {sv.x, sv.y, sv.z, sv.w};
 #pragma unroll
-                                    for (int i = 0; i < 4; ++i) {
-                                        if (col + i < n_valid) {
-                                            if (p.atomic) atomicAdd(fd + i, e4[i]);
-                                            else fd[i] = e4[i];
+                                        for (int i = 0; i < 4; ++i) {
+                                            if (col + i < n_valid) {
+                                                if (p.atomic) atomicAdd(fd + i, e4[i]);
+                                                else fd[i] = e4[i];
+                                            }
                                         }
                                     }
-                                }
-                            } else {
-                                uint4 sv = *reinterpret_cast<const uint4 *>(src);
-                                if (full) {
-                                    if (p.atomic) {                   // D += product (16-bit outputs: read-modify-write, no split-K)
-                                        const uint4 o = *reinterpret_cast<const uint4 *>(dst);
-                                        sv = make_uint4(sum2<TOut>(o.x, sv.x), sum2<TOut>(o.y, sv.y), sum2<TOut>(o.z, sv.z), sum2<TOut>(o.w, sv.w));
-                                    }
-                                    *reinterpret_cast<uint4 *>(dst) = sv;
                                 } else {
-                                    const TOut *se = reinterpret_cast<const TOut *>(&sv);
+                                    uint4 sv = *reinterpret_cast<const uint4 *>(src);
+                                    if (full16) {
+                                        if (p.atomic) {                   // D += product (16-bit outputs: read-modify-write, no split-K)
+                                            const uint4 o = *reinterpret_cast<const uint4 *>(dst);
+                                            sv = make_uint4(sum2<TOut>(o.x, sv.x), sum2<TOut>(o.y, sv.y), sum2<TOut>(o.z, sv.z), sum2<TOut>(o.w, sv.w));
+                                        }
+                                        *reinterpret_cast<uint4 *>(dst) = sv;
+                                    } else {
+                                        const TOut *se = reinterpret_cast<const TOut *>(&sv);
 #pragma unroll
-                                    for (int i = 0; i < kVec; ++i) {
-                                        if (col + i < n_valid) {
-                                            const float o = p.atomic ? static_cast<float>(dst[i]) + static_cast<float>(se[i]) : static_cast<float>(se[i]);
-                                            dst[i] = static_cast<TOut>(o);
+                                        for (int i = 0; i < kVec; ++i) {
+                                            if (col + i < n_valid) {
+                                                const float o = p.atomic ? static_cast<float>(dst[i]) + static_cast<float>(se[i]) : static_cast<float>(se[i]);
+                                                dst[i] = static_cast<TOut>(o);
+                                            }
                                         }
                                     }
                                 }
                             }
                         }
+                        __syncwarp();
                     }
-                    __syncwarp();
-                    if (p.prof && warp == 2 && lane == 0) atomicAdd(p.prof + 10, (unsigned long long)(clock64() - tq2));
                 }
             }
-            if (p.prof && warp == 2 && lane == 0) atomicAdd(p.prof + 11, (unsigned long long)(clock64() - t_tile0));
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[as]);      // accumulator buffer drained: the MMA warp may reuse it
+            if (p.prof && warp == 4 && lane == 0) atomicAdd(p.prof + 11, (unsigned long long)(clock64() - t_tile0));
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (p.prof && threadIdx.x == 0) atomicAdd(p.prof + 7, (unsigned long long)(clock64() - t_start));
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(p.tmem_cols) : "memory");
+        if (p.prof && warp == 4 && lane == 0) atomicAdd(p.prof + 7, (unsigned long long)(clock64() - t_start));
     }
 }
 
@@ -455,9 +423,12 @@ cudaError_t encode_2d(CUtensorMap *m, const void *base, int dtype, uint64_t inne
 
 }  // namespace
 
+// the narrowest instantiated tile that covers N (256 for anything wider)
 int gemm_pick_bn(int N) {
-    if (N >= 256) return 256;
-    return ((N + 15) / 16) * 16;
+    for (int bn : {16, 32, 48, 64, 96, 128, 192}) {
+        if (N <= bn) return bn;
+    }
+    return 256;
 }
 
 cudaError_t gemm_tc_launch(GemmP p, const void *A, int64_t lda, const void *B, int64_t ldb, cudaStream_t st, const char **where) {
@@ -472,21 +443,19 @@ cudaError_t gemm_tc_launch(GemmP p, const void *A, int64_t lda, const void *B, i
         cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     }
     if (p.BN <= 0) p.BN = gemm_pick_bn(p.N);
+    if (p.BN != gemm_pick_bn(p.BN)) return cudaErrorInvalidValue;      // a preset BN must be one of the instantiated tiles
     const int BN = p.BN;
     const size_t b_tile = p.b_mn ? (size_t)((BN + 63) / 64) * 8192 : (size_t)BN * 128;
     const size_t stage_bytes = (size_t)kBM * 128 + ((b_tile + 1023) & ~(size_t)1023);
-    const size_t fixed = 1024 + kEpiWarps * 32 * 144 + (2 * kMaxStages + 4) * 8 + 16;
+    const size_t fixed = 1024 + kStagingBytes + 2 * kMaxStages * 8;
     int stages = (int)(((size_t)max_smem - fixed) / stage_bytes);
     if (stages > kMaxStages) stages = kMaxStages;
     const int kb_total = (p.K + kBK - 1) / kBK;
     if (stages < 2) return cudaErrorInvalidConfiguration;
     p.stages = stages;
-    int cols = 32;
-    while (cols < 2 * BN + ((BN & 31) ? 16 : 0)) cols <<= 1;   // the epilogue reads 32 columns at a time: keep its last read inside the allocation
-    p.tmem_cols = cols;
     if (p.split_k < 1) p.split_k = 1;
     if (p.split_k > kb_total) p.split_k = kb_total;
-    {   // no K slice may be empty: an accumulator that no MMA wrote would be added as is
+    {   // no K slice may be empty: an accumulator that no wgmma wrote would be added as is
         const int kb_per = (kb_total + p.split_k - 1) / p.split_k;
         p.split_k = (kb_total + kb_per - 1) / kb_per;
     }
@@ -515,23 +484,37 @@ cudaError_t gemm_tc_launch(GemmP p, const void *A, int64_t lda, const void *B, i
 
     const int m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + BN - 1) / BN;
     const long n_work = (long)m_tiles * n_tiles * p.split_k;
-    const int ctas_per_sm = smem * 2 + 2048 <= (size_t)228 * 1024 && cols <= 256 ? 2 : 1;
-    const int grid = (int)(n_work < (long)sms * ctas_per_sm ? n_work : (long)sms * ctas_per_sm);
-#define SMB_GEMM_LAUNCH(T)                                                                                                  \
+    const int grid = (int)(n_work < (long)sms ? n_work : (long)sms);
+#define SMB_GEMM_LAUNCH(TIn, TOut, kBN)                                                                                     \
     do {                                                                                                                    \
-        static size_t set = 0;                                                                                              \
+        static bool set = false;                                                                                            \
         *where = "cudaFuncSetAttribute";                                                                                    \
-        if (smem > set) {                                                                                                   \
-            e = cudaFuncSetAttribute(gemm_tc_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem);        \
+        if (!set) {                                                                                                         \
+            e = cudaFuncSetAttribute(gemm_tc_kernel<TIn, TOut, kBN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem); \
             if (e != cudaSuccess) return e;                                                                                 \
-            set = (size_t)max_smem;                                                                                         \
+            set = true;                                                                                                     \
         }                                                                                                                   \
         *where = "kernel launch";                                                                                           \
-        gemm_tc_kernel<T><<<grid, kThreads, smem, st>>>(tmA, tmB, p);                                                       \
+        gemm_tc_kernel<TIn, TOut, kBN><<<grid, kThreads, smem, st>>>(tmA, tmB, p);                                          \
     } while (0)
-    if (p.out_dtype == 0) SMB_GEMM_LAUNCH(float);
-    else if (p.out_dtype == 1) SMB_GEMM_LAUNCH(__half);
-    else SMB_GEMM_LAUNCH(__nv_bfloat16);
+#define SMB_GEMM_TYPES(kBN)                                                                                                 \
+    do {                                                                                                                    \
+        if (p.dtype == 1 && p.out_dtype == 0) SMB_GEMM_LAUNCH(__half, float, kBN);                                          \
+        else if (p.dtype == 1) SMB_GEMM_LAUNCH(__half, __half, kBN);                                                        \
+        else if (p.out_dtype == 0) SMB_GEMM_LAUNCH(__nv_bfloat16, float, kBN);                                              \
+        else SMB_GEMM_LAUNCH(__nv_bfloat16, __nv_bfloat16, kBN);                                                            \
+    } while (0)
+    switch (BN) {
+        case 16: SMB_GEMM_TYPES(16); break;
+        case 32: SMB_GEMM_TYPES(32); break;
+        case 48: SMB_GEMM_TYPES(48); break;
+        case 64: SMB_GEMM_TYPES(64); break;
+        case 96: SMB_GEMM_TYPES(96); break;
+        case 128: SMB_GEMM_TYPES(128); break;
+        case 192: SMB_GEMM_TYPES(192); break;
+        default: SMB_GEMM_TYPES(256); break;
+    }
+#undef SMB_GEMM_TYPES
 #undef SMB_GEMM_LAUNCH
     count_launch();
     return cudaGetLastError();

@@ -1,4 +1,4 @@
-// Fused InstanceNorm3d (+ optional second operand, + ReLU / LeakyReLU) forward / backward for sm_100a,
+// Fused InstanceNorm3d (+ optional second operand, + ReLU / LeakyReLU) forward / backward for sm_90a,
 // on channels-last activations viewed as (batch, spatial, channels).
 //
 // Replaces the reference's nn.InstanceNorm3d(affine=False, eps=1e-5) + activation + residual-add chains:
@@ -7,7 +7,7 @@
 //                                                                      monai/networks/blocks/dynunet_block.py:98-111
 //   downsample / norm{i}   IN(x)                                       segmamba.py:147,171
 // which the reference runs as ATen batch_norm kernels in fp32 plus separate elementwise kernels (38 % of its
-// training step on B200, profiles/r1_launches_train_step_v1.csv).  These are pure HBM streaming ops:
+// training step).  These are pure HBM streaming ops:
 //   forward : 1 read for the statistics + 1 read + 1 write for the apply     (per operand)
 //   backward: reads dy, x (, x2) twice (sums, then apply), writes dx (, dx2)
 // Mapping: a CTA owns a contiguous range of rows (voxels); thread (r, cv) owns the 16-byte column vector cv of
@@ -22,9 +22,8 @@ constexpr int kNormThreads = 256;
 #ifndef SMB_IN_FWD_MINB
 #define SMB_IN_FWD_MINB 3
 #endif
-// backward kernels, by second-operand mode (slot r2o, tools/norm_bench.py: at (2, 48, 128^3) bf16 the single-operand backward goes
-// 0.535 -> 0.476 ms with 5 resident CTAs and one row in flight, the raw-residual one 0.625 -> 0.567 ms with 4; the two-norm one
-// spills beyond 2 and stays there)
+// backward kernels, by second-operand mode (tools/norm_bench.py sweeps them; the values below were not re-swept on H100; the
+// two-norm one spills beyond 2 and stays there)
 #ifndef SMB_IN_BWD_MINB0
 #define SMB_IN_BWD_MINB0 5
 #endif

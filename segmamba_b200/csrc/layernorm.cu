@@ -1,10 +1,10 @@
 // Fused LayerNorm over the channel axis of the (tokens, C) matrix that feeds every Mamba mixer, forward and backward,
-// for sm_100a.
+// for sm_90a.
 //
 // Replaces nn.LayerNorm(dim) in MambaLayer.forward (model_segmamba/segmamba.py:54,70): under autocast the reference runs
 // it as ATen fp32 kernels (bf16 -> fp32 input cast, vectorized_layer_norm_kernel, fp32 -> bf16 cast before in_proj; in
-// backward layer_norm_grad_input + GammaBetaBackward, which alone takes 0.23 ms per call at (524288, 48)):
-// 4.5 ms of the 102 ms training step (profiles/r1_launches_train_step_v3.csv).  The op is a pure HBM stream:
+// backward layer_norm_grad_input + GammaBetaBackward).
+// The op is a pure HBM stream:
 //   forward : read x, write y                      2 * s * rows * C bytes
 //   backward: read x, dy, write dx (+ C floats)    3 * s * rows * C bytes   (statistics are recomputed, nothing is saved)
 // Mapping: a row (token) is C/V 16-byte vectors; LPR = the next power of two >= C/V lanes (at most 32) own one row, each
@@ -224,7 +224,7 @@ template <typename T, int VPL>
 static cudaError_t ln_launch(const LnP &p, bool bwd, int lpr, cudaStream_t st) {
     const int rows_per_cta = kLnWarps * (32 / lpr);
     int64_t ctas = (p.rows + rows_per_cta - 1) / rows_per_cta;
-    const int64_t cap = 148 * 8;                                  // persistent-style grid: 8 CTAs of 8 warps per SM at most
+    const int64_t cap = 132 * 8;                                  // persistent-style grid: 8 CTAs of 8 warps per SM at most
     if (ctas > cap) ctas = cap;
     if (!bwd) {
         ln_fwd_kernel<T, VPL><<<(unsigned)ctas, kLnThreads, 0, st>>>(p, lpr);

@@ -23,7 +23,7 @@ inline void norm_plan(int batch, int channels, int64_t spatial, int elem_bytes, 
     const int V = 16 / elem_bytes;
     const int CV = channels / V;
     const int RB = 256 / CV;
-    const int64_t target = (148 * 8 + batch - 1) / batch;
+    const int64_t target = (132 * 8 + batch - 1) / batch;
     int64_t rows = (spatial + target - 1) / target;
     if (rows < (int64_t)RB * 8) rows = (int64_t)RB * 8;
     *rows_per_cta = rows;

@@ -1,4 +1,4 @@
-// Backward selective scan for sm_100a: chunk-parallel, three passes over 256-position chunks.
+// Backward selective scan for sm_90a: chunk-parallel, three passes over 256-position chunks.
 //
 //   R1  scan_bwd_ragg_kernel  lane-per-channel reverse walk of each chunk with zero incoming adjoint:
 //                             (P = prod a, Mloc = adjoint at the chunk start)                     [1 ex2 / update]
@@ -241,9 +241,9 @@ __global__ void __launch_bounds__(kBwdWarps * 32) scan_bwd_main_kernel(const Sca
             float2 a2[kRun / 2], bb2[kRun / 2], gc2[kRun / 2], hs2[kRun / 2], lam2[kRun / 2];
 #pragma unroll
             for (int j = 0; j < kRun / 2; ++j) {
-                a2[j] = ex2x2_mufu(__fmul2_rn(dt2[j], A2n2));
-                bb2[j] = __fmul2_rn(dtu2[j], Bv2[j]);
-                gc2[j] = __fmul2_rn(g2[j], Cv2[j]);
+                a2[j] = ex2x2_mufu(fmul2(dt2[j], A2n2));
+                bb2[j] = fmul2(dtu2[j], Bv2[j]);
+                gc2[j] = fmul2(g2[j], Cv2[j]);
             }
             // lane aggregates of the forward recurrence (sequential over the 8 positions)
             float Aagg = 1.f, Hagg = 0.f;
@@ -292,14 +292,14 @@ __global__ void __launch_bounds__(kBwdWarps * 32) scan_bwd_main_kernel(const Sca
             float2 dA2 = f2(0.f, 0.f);
 #pragma unroll
             for (int j = 0; j < kRun / 2; ++j) {
-                yy2[j] = __ffma2_rn(Cv2[j], hs2[j], yy2[j]);
-                dC2[j] = __fmul2_rn(g2[j], hs2[j]);
-                dB2[j] = __fmul2_rn(lam2[j], dtu2[j]);
-                sLB2[j] = __ffma2_rn(lam2[j], Bv2[j], sLB2[j]);
-                const float2 hm = __ffma2_rn(bb2[j], f2(-1.f, -1.f), hs2[j]);     // h - b = a h_prev
-                const float2 qv = __fmul2_rn(lam2[j], hm);
-                dA2 = __ffma2_rn(dt2[j], qv, dA2);
-                sAq2[j] = __ffma2_rn(A2n2, qv, sAq2[j]);
+                yy2[j] = ffma2(Cv2[j], hs2[j], yy2[j]);
+                dC2[j] = fmul2(g2[j], hs2[j]);
+                dB2[j] = fmul2(lam2[j], dtu2[j]);
+                sLB2[j] = ffma2(lam2[j], Bv2[j], sLB2[j]);
+                const float2 hm = ffma2(bb2[j], f2(-1.f, -1.f), hs2[j]);     // h - b = a h_prev
+                const float2 qv = fmul2(lam2[j], hm);
+                dA2 = ffma2(dt2[j], qv, dA2);
+                sAq2[j] = ffma2(A2n2, qv, sAq2[j]);
             }
             const float dAacc = warp_sum(dA2.x + dA2.y);          // dA_n = sum_t lambda dt (h - b)
             if (lane == 0) atomicAdd(p.dA + (int64_t)d * N + n, dAacc);
@@ -654,13 +654,13 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 2) scan_bwd_sweep_kernel(co
                         const int m = 2 * jn + hh;
                         const float2 Bp = hh ? f2(b4.z, b4.w) : f2(b4.x, b4.y);
                         const float2 Cp = hh ? f2(c4.z, c4.w) : f2(c4.x, c4.y);
-                        const float2 a = ex2x2_mufu(__fmul2_rn(dt2, A2[m]));
-                        const float2 lam = __ffma2_rn(g2, Cp, mu[m]);
-                        mu[m] = __fmul2_rn(a, lam);
-                        yacc = __ffma2_rn(Cp, hcur[m], yacc);
-                        vC[m] = __fmul2_rn(g2, hcur[m]);
-                        vB[m] = __fmul2_rn(lam, dtu2);
-                        slb = __ffma2_rn(lam, Bp, slb);
+                        const float2 a = ex2x2_mufu(fmul2(dt2, A2[m]));
+                        const float2 lam = ffma2(g2, Cp, mu[m]);
+                        mu[m] = fmul2(a, lam);
+                        yacc = ffma2(Cp, hcur[m], yacc);
+                        vC[m] = fmul2(g2, hcur[m]);
+                        vB[m] = fmul2(lam, dtu2);
+                        slb = ffma2(lam, Bp, slb);
                     }
                 }
                 // ---- reduce vB / vC over the 32 channels of this warp: transpose through shared memory ----
@@ -674,9 +674,9 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 2) scan_bwd_sweep_kernel(co
 #pragma unroll
                 for (int m = 0; m < N / 2; ++m) {
                     const float2 hpv = stash_cvt(hp[m]);
-                    const float2 qm = __fmul2_rn(mu[m], hpv);                // lambda_t a_t h_{t-1}
-                    dA2[m] = __ffma2_rn(dt2, qm, dA2[m]);
-                    saq = __ffma2_rn(A2[m], qm, saq);
+                    const float2 qm = fmul2(mu[m], hpv);                // lambda_t a_t h_{t-1}
+                    dA2[m] = ffma2(dt2, qm, dA2[m]);
+                    saq = ffma2(A2[m], qm, saq);
                     hcur[m] = hpv;
                 }
                 const float y = fmaf(Dv, uv, yacc.x + yacc.y);

@@ -1,8 +1,8 @@
 // Backward selective scan, pass R3, second generation (opt-in: SMB_R3_V2=1; emulator-validated, first hardware run pending).
 //
 // Same algorithm, operands, outputs and launch geometry as scan_bwd_main_kernel (scan_bwd.cu: warp == channel, lane == run of
-// 8 positions, CTA == 8 channels of one 256-position chunk) -- R3 is issue-bound (57 % of the issue slots busy at 25 %
-// occupancy, profiles/r1_ncu_kernels_final_summary.txt), so this version removes instructions, not memory traffic.  Per
+// 8 positions, CTA == 8 channels of one 256-position chunk) -- this version removes instructions, not memory
+// traffic.  Per
 // (state, 8 positions, lane), counted in SASS with tools/sass_loops.py: 318 -> see DESIGN.md 3.2.
 //   * Kogge-Stone steps use the shuffle's own in-range predicate (shfl.sync ... d|p) on the combine, so the step is
 //     2 SHFL + 1 FFMA + 1 FMUL with no ISETP / FSEL; the last step drops the span product altogether.
@@ -125,10 +125,10 @@ __device__ __forceinline__ void r3_state(const float *__restrict__ rowB, const f
     float2 a2[kRun / 2], bb2[kRun / 2], gc2[kRun / 2], agc2[kRun / 2], hs2[kRun / 2], lam2[kRun / 2];
 #pragma unroll
     for (int j = 0; j < kRun / 2; ++j) {
-        a2[j] = ex2x2_mufu(__fmul2_rn(dt2[j], A2n2));
-        bb2[j] = __fmul2_rn(dtu2[j], Bv2[j]);
-        gc2[j] = __fmul2_rn(g2[j], Cv2[j]);
-        agc2[j] = __fmul2_rn(a2[j], gc2[j]);
+        a2[j] = ex2x2_mufu(fmul2(dt2[j], A2n2));
+        bb2[j] = fmul2(dtu2[j], Bv2[j]);
+        gc2[j] = fmul2(g2[j], Cv2[j]);
+        agc2[j] = fmul2(a2[j], gc2[j]);
     }
     if constexpr (kDense) {
         float h = h_in;
@@ -142,7 +142,7 @@ __device__ __forceinline__ void r3_state(const float *__restrict__ rowB, const f
         for (int j = kRun / 2 - 1; j >= 0; --j) {
             const float my = m; m = fmaf(a2[j].y, m, agc2[j].y);
             const float mx = m; m = fmaf(a2[j].x, m, agc2[j].x);
-            lam2[j] = __fadd2_rn(gc2[j], f2(mx, my));      // lambda_i = g_i C_i + mu_{i+1}
+            lam2[j] = fadd2(gc2[j], f2(mx, my));      // lambda_i = g_i C_i + mu_{i+1}
         }
     } else {
     const float Aagg = ex2(A2n * sumdt);               // product of the run's eight decays
@@ -182,7 +182,7 @@ __device__ __forceinline__ void r3_state(const float *__restrict__ rowB, const f
         for (int j = kRun / 2 - 1; j >= 0; --j) {
             const float my = m; m = fmaf(a2[j].y, m, agc2[j].y);
             const float mx = m; m = fmaf(a2[j].x, m, agc2[j].x);
-            lam2[j] = __fadd2_rn(gc2[j], f2(mx, my));  // lambda_i = g_i C_i + mu_{i+1}
+            lam2[j] = fadd2(gc2[j], f2(mx, my));  // lambda_i = g_i C_i + mu_{i+1}
         }
     }
     }   // !kDense
@@ -190,14 +190,14 @@ __device__ __forceinline__ void r3_state(const float *__restrict__ rowB, const f
     float2 dA2 = f2(0.f, 0.f), dB2[kRun / 2], dC2[kRun / 2];
 #pragma unroll
     for (int j = 0; j < kRun / 2; ++j) {
-        yy2[j] = __ffma2_rn(Cv2[j], hs2[j], yy2[j]);
-        dC2[j] = __fmul2_rn(g2[j], hs2[j]);
-        dB2[j] = __fmul2_rn(lam2[j], dtu2[j]);
-        sLB2[j] = __ffma2_rn(lam2[j], Bv2[j], sLB2[j]);
-        const float2 hm = __ffma2_rn(bb2[j], f2(-1.f, -1.f), hs2[j]);     // h - b = a h_prev
-        const float2 qv = __fmul2_rn(lam2[j], hm);
-        dA2 = __ffma2_rn(dt2[j], qv, dA2);
-        sAq2[j] = __ffma2_rn(A2n2, qv, sAq2[j]);
+        yy2[j] = ffma2(Cv2[j], hs2[j], yy2[j]);
+        dC2[j] = fmul2(g2[j], hs2[j]);
+        dB2[j] = fmul2(lam2[j], dtu2[j]);
+        sLB2[j] = ffma2(lam2[j], Bv2[j], sLB2[j]);
+        const float2 hm = ffma2(bb2[j], f2(-1.f, -1.f), hs2[j]);     // h - b = a h_prev
+        const float2 qv = fmul2(lam2[j], hm);
+        dA2 = ffma2(dt2[j], qv, dA2);
+        sAq2[j] = ffma2(A2n2, qv, sAq2[j]);
     }
     *sda_n = dA2.x + dA2.y;
     *reinterpret_cast<float4 *>(myB) = make_float4(dB2[0].x, dB2[0].y, dB2[1].x, dB2[1].y);
@@ -410,14 +410,14 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
             float4 v[kW];
 #pragma unroll
             for (int w2 = 0; w2 < kW; ++w2) v[w2] = *reinterpret_cast<const float4 *>(rsrc + w2 * kPad);
-            const float2 lo = __fadd2_rn(__fadd2_rn(__fadd2_rn(f2(v[0].x, v[0].y), f2(v[1].x, v[1].y)),
-                                                    __fadd2_rn(f2(v[2].x, v[2].y), f2(v[3].x, v[3].y))),
-                                         __fadd2_rn(__fadd2_rn(f2(v[4].x, v[4].y), f2(v[5].x, v[5].y)),
-                                                    __fadd2_rn(f2(v[6].x, v[6].y), f2(v[7].x, v[7].y))));
-            const float2 hi = __fadd2_rn(__fadd2_rn(__fadd2_rn(f2(v[0].z, v[0].w), f2(v[1].z, v[1].w)),
-                                                    __fadd2_rn(f2(v[2].z, v[2].w), f2(v[3].z, v[3].w))),
-                                         __fadd2_rn(__fadd2_rn(f2(v[4].z, v[4].w), f2(v[5].z, v[5].w)),
-                                                    __fadd2_rn(f2(v[6].z, v[6].w), f2(v[7].z, v[7].w))));
+            const float2 lo = fadd2(fadd2(fadd2(f2(v[0].x, v[0].y), f2(v[1].x, v[1].y)),
+                                                    fadd2(f2(v[2].x, v[2].y), f2(v[3].x, v[3].y))),
+                                         fadd2(fadd2(f2(v[4].x, v[4].y), f2(v[5].x, v[5].y)),
+                                                    fadd2(f2(v[6].x, v[6].y), f2(v[7].x, v[7].y))));
+            const float2 hi = fadd2(fadd2(fadd2(f2(v[0].z, v[0].w), f2(v[1].z, v[1].w)),
+                                                    fadd2(f2(v[2].z, v[2].w), f2(v[3].z, v[3].w))),
+                                         fadd2(fadd2(f2(v[4].z, v[4].w), f2(v[5].z, v[5].w)),
+                                                    fadd2(f2(v[6].z, v[6].w), f2(v[7].z, v[7].w))));
             if (p.dbg & 1) {
                 if (lo.x == 1.2345e33f) rdst[0] = hi.y;      // keep the sums live
             } else if (vec_ok && rpos0 + 3 < L) {
@@ -508,12 +508,12 @@ template <typename T, int N, bool kHasZ>
 cudaError_t launch_main2(const ScanP &p, cudaStream_t st) {
     const size_t sm = R3Smem<N>::kBytes;
     cudaError_t e;
-    // octets per CTA: as many as keeps >= ~4 CTAs per resident slot (2 x 148) in the grid
+    // octets per CTA: as many as keeps >= ~4 CTAs per resident slot (8 x 132 SMs) in the grid
     const int opg = (p.dim_per_group + kW - 1) / kW;
     ScanP q = p;
     {
         const long total = (long)p.nck * opg * p.G * p.batch;
-        long opc = total / 1184;
+        long opc = total / 1056;
         if (opc < 1) opc = 1;
         if (opc > opg) opc = opg;
         const char *e = getenv("SMB_R3_OPC");            // A/B switch: octets per CTA (1 = one CTA per octet, as in round 1)

@@ -1,4 +1,4 @@
-// Forward selective scan for sm_100a: lane-per-channel, three passes.
+// Forward selective scan for sm_90a: lane-per-channel, three passes.
 //
 //   pass 1  scan_fwd_agg_kernel   per (batch, 32-channel tile, segment): zero-initialised recurrence over the
 //                                 segment -> aggregate (P = prod a, H = state) per state          [1 ex2 / update]
@@ -369,7 +369,7 @@ cudaError_t x_finalize_launch(const ScanP &p, int N, float *x, cudaStream_t st) 
 cudaError_t scan_fwd_dispatch(const ScanP &p, int dtype, int N, bool has_z, float *x, cudaStream_t st) {
     {   // 16-bit activations: software-pipelined kernels, tiles staged by TMA (mode 2; falls back to cp.async staging, mode 1,
         // when no tensor map can describe the operands).  SMB_FWD_V2=0 selects the single-buffered kernels below, =1 the
-        // cp.async staging -- A/B switches (profiles/r2a_microbench_ab.md), read per call.
+        // cp.async staging -- A/B switches, read per call.
         const char *v2 = getenv("SMB_FWD_V2");
         const int mode = (v2 && v2[0] >= '0' && v2[0] <= '2') ? v2[0] - '0' : 2;
         if (dtype != 0 && mode) return scan_fwd_v2_dispatch(p, dtype, N, has_z, x, mode, st);

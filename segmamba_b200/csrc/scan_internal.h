@@ -80,18 +80,17 @@ __device__ __forceinline__ WorkItem decode_work(const ScanP &p, int w) {
 }
 
 // Segment length heuristic (host): largest S in {seg_min .. 2048} that still yields >= 24 warps per SM (two waves at the
-// 12-warp residency the kernels reach) on a 148-SM B200; S divides 2048 so the reference's 2048-position chunk states fall on
+// 12-warp residency the kernels reach) on the 132 SMs of an H100; S divides 2048 so the reference's 2048-position chunk states fall on
 // segment ends, and divides or is a multiple of kCkpt so checkpoints fall on tile boundaries of exactly one segment.
-// Shortest segment: one 32-position tile, so that the small late-stage problems (L = 4096 / 512) still spread over the chip
-// (stage 3 forward: 0.134 ms with 256-position segments, 0.052 ms with 32; profiles/r2a_microbench_ab.md).  SMB_SEG_MIN = 64 /
-// 128 / 256 is the A/B switch (read per call).
+// Shortest segment: one 32-position tile, so that the small late-stage problems (L = 4096 / 512) still spread over the chip.
+// SMB_SEG_MIN = 64 / 128 / 256 is the A/B switch (read per call).
 inline int seg_min() {
     const char *e = getenv("SMB_SEG_MIN");
     const int v = e ? atoi(e) : 32;
     return (v == 64 || v == 128 || v == 256) ? v : 32;
 }
 inline int plan_segment(int batch, int n_tiles, int L) {
-    const long target = 148L * 24;
+    const long target = 132L * 24;
     const int smin = seg_min();
     int S = 2048;
     while (S > smin && (long)batch * n_tiles * ((L + S - 1) / S) < target) S >>= 1;

@@ -14,10 +14,10 @@ template <int N, int QL, int JN>
 __device__ __forceinline__ void scan_step_agg_chunk(const float *s_B, float2 dt2, float2 du2, const float2 (&A2)[N / 2],
                                                     float2 (&h)[N / 2]) {
     const float4 b4 = bc_read4_c<N, QL, JN>(s_B);
-    const float2 a0 = decay2<2 * JN>(__fmul2_rn(dt2, A2[2 * JN]));
-    const float2 a1 = decay2<2 * JN + 1>(__fmul2_rn(dt2, A2[2 * JN + 1]));
-    h[2 * JN] = __ffma2_rn(a0, h[2 * JN], __fmul2_rn(du2, f2(b4.x, b4.y)));
-    h[2 * JN + 1] = __ffma2_rn(a1, h[2 * JN + 1], __fmul2_rn(du2, f2(b4.z, b4.w)));
+    const float2 a0 = decay2<2 * JN>(fmul2(dt2, A2[2 * JN]));
+    const float2 a1 = decay2<2 * JN + 1>(fmul2(dt2, A2[2 * JN + 1]));
+    h[2 * JN] = ffma2(a0, h[2 * JN], fmul2(du2, f2(b4.x, b4.y)));
+    h[2 * JN + 1] = ffma2(a1, h[2 * JN + 1], fmul2(du2, f2(b4.z, b4.w)));
 }
 template <int N, int QL>
 __device__ __forceinline__ void scan_step_agg(const float *s_B, float2 dt2, float2 du2, const float2 (&A2)[N / 2],
@@ -34,12 +34,12 @@ __device__ __forceinline__ void scan_step_main_chunk(const float *s_B, const flo
                                                      const float2 (&A2)[N / 2], float2 (&h)[N / 2], float2 &y) {
     const float4 b4 = bc_read4_c<N, QL, JN>(s_B);
     const float4 c4 = bc_read4_c<N, QL, JN>(s_C);
-    const float2 a0 = decay2<2 * JN>(__fmul2_rn(dt2, A2[2 * JN]));
-    const float2 a1 = decay2<2 * JN + 1>(__fmul2_rn(dt2, A2[2 * JN + 1]));
-    h[2 * JN] = __ffma2_rn(a0, h[2 * JN], __fmul2_rn(du2, f2(b4.x, b4.y)));
-    h[2 * JN + 1] = __ffma2_rn(a1, h[2 * JN + 1], __fmul2_rn(du2, f2(b4.z, b4.w)));
-    y = __ffma2_rn(f2(c4.x, c4.y), h[2 * JN], y);
-    y = __ffma2_rn(f2(c4.z, c4.w), h[2 * JN + 1], y);
+    const float2 a0 = decay2<2 * JN>(fmul2(dt2, A2[2 * JN]));
+    const float2 a1 = decay2<2 * JN + 1>(fmul2(dt2, A2[2 * JN + 1]));
+    h[2 * JN] = ffma2(a0, h[2 * JN], fmul2(du2, f2(b4.x, b4.y)));
+    h[2 * JN + 1] = ffma2(a1, h[2 * JN + 1], fmul2(du2, f2(b4.z, b4.w)));
+    y = ffma2(f2(c4.x, c4.y), h[2 * JN], y);
+    y = ffma2(f2(c4.z, c4.w), h[2 * JN + 1], y);
 }
 template <int N, int QL>
 __device__ __forceinline__ float scan_step_main(const float *s_B, const float *s_C, float2 dt2, float2 du2,
@@ -51,7 +51,7 @@ __device__ __forceinline__ float scan_step_main(const float *s_B, const float *s
         scan_step_main_chunk<N, QL, (N == 16 ? 2 : 0)>(s_B, s_C, dt2, du2, A2, h, ya);
         scan_step_main_chunk<N, QL, (N == 16 ? 3 : 1)>(s_B, s_C, dt2, du2, A2, h, yb);
     }
-    const float2 ys = __fadd2_rn(ya, yb);
+    const float2 ys = fadd2(ya, yb);
     return ys.x + ys.y;
 }
 
@@ -85,10 +85,10 @@ template <int N, int QL, int JN>
 __device__ __forceinline__ void ragg_step_chunk(const float *s_C, float2 dt2, float2 g2, const float2 (&A2)[N / 2],
                                                 float2 (&mu)[N / 2]) {
     const float4 c4 = bc_read4_c<N, QL, JN>(s_C);
-    const float2 a0 = decay2<2 * JN>(__fmul2_rn(dt2, A2[2 * JN]));
-    const float2 a1 = decay2<2 * JN + 1>(__fmul2_rn(dt2, A2[2 * JN + 1]));
-    mu[2 * JN] = __fmul2_rn(a0, __ffma2_rn(g2, f2(c4.x, c4.y), mu[2 * JN]));
-    mu[2 * JN + 1] = __fmul2_rn(a1, __ffma2_rn(g2, f2(c4.z, c4.w), mu[2 * JN + 1]));
+    const float2 a0 = decay2<2 * JN>(fmul2(dt2, A2[2 * JN]));
+    const float2 a1 = decay2<2 * JN + 1>(fmul2(dt2, A2[2 * JN + 1]));
+    mu[2 * JN] = fmul2(a0, ffma2(g2, f2(c4.x, c4.y), mu[2 * JN]));
+    mu[2 * JN + 1] = fmul2(a1, ffma2(g2, f2(c4.z, c4.w), mu[2 * JN + 1]));
 }
 template <int N, int QL>
 __device__ __forceinline__ void ragg_step(const float *s_C, float2 dt2, float2 g2, const float2 (&A2)[N / 2],

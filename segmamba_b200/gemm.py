@@ -1,4 +1,4 @@
-"""Pointwise contractions on the tensor-core GEMM of libsegmamba_b200 (smb_gemm: TMA -> tcgen05.mma -> tensor memory).
+"""Pointwise contractions on the tensor-core GEMM of libsegmamba_b200 (smb_gemm: TMA -> wgmma, accumulator in registers).
 
 ``gemm(a, b, ...)`` computes  D[M, N] = epilogue(A[M, K] . B[N, K]^T)  from 2-D views of 16-bit tensors: an operand whose
 last axis is contiguous is passed K-major, an operand whose FIRST axis is contiguous (a transposed view) is passed MN-major,
@@ -20,11 +20,10 @@ from . import _lib
 
 EPI_NONE, EPI_BIAS_N, EPI_BIAS_N_GELU, EPI_BIAS_M = 0, 1, 2, 3
 
-# Which products of the model run on the native kernel (measured per shape against the library on B200, profiles/r2j_gemm_bench.md):
+# Which products of the model run on the native kernel (the split is not re-measured per shape on H100):
 #   "auto" (default)  the products that contract over the token axis -- every weight gradient of the mixer (dW of in_proj /
-#                     x_proj / dt_proj / out_proj; K = 65 536 ... 524 288 tokens split over the SMs with fp32 atomics): native
-#                     1.07 - 1.40 x the library; the activation-sized products (output = tokens x channels), where the kernel
-#                     reaches 0.4 - 0.8 x the library, stay library calls, as in the reference;
+#                     x_proj / dt_proj / out_proj; K = 65 536 ... 524 288 tokens split over the SMs with fp32 atomics); the
+#                     activation-sized products (output = tokens x channels) stay library calls, as in the reference;
 #   "all"             every pointwise contraction and 1x1x1 convolution;      "off"  none.
 MODE = os.environ.get("SMB_GEMM", "auto")
 SPLIT_TOKENS = 16384     # contraction length from which the split-K path is used (and wins)
@@ -89,7 +88,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, bias: torch.Tensor | None = None, epi
 
 def _split_k_for(tokens: int) -> int:
     """weight-gradient products contract over the token axis: one K slice per ~SM, at least 512 tokens each."""
-    return max(1, min(148, tokens // 512))
+    return max(1, min(132, tokens // 512))
 
 
 class _Linear(torch.autograd.Function):

@@ -1,14 +1,14 @@
 """Whole-step CUDA-graph capture for the SegMamba training step.
 
-One training step of the default model enqueues ~4 500 kernels (cuDNN / cuBLAS / ATen / native); at ~100 ms of GPU time the
-host needs ~65 ms just to launch them (bench.py: host_enqueue_ms_per_step), so the step is one kernel-speedup away from
-being launch-bound.  ``GraphedTrainStep`` captures forward + loss + backward + gradient clipping + optimizer step once and
+One training step of the default model enqueues several thousand kernels (cuDNN / cuBLAS / ATen / native), and the host's time
+to launch them (bench.py: host_enqueue_ms_per_step) is a large fraction of the step's GPU time, so kernel speed-ups push the
+step towards being launch-bound.  ``GraphedTrainStep`` captures forward + loss + backward + gradient clipping + optimizer step once and
 replays it with a single ``cudaGraphLaunch`` per step (static input / label buffers, private memory pool).  All native
 kernels are capture-safe by construction: they only enqueue work on the current stream and allocate through the PyTorch
 caching allocator.
 
 This replaces nothing in the reference (its trainer launches eagerly, light_training/trainer.py:422-483); it is the
-"CUDA graphs instead of a tracing compiler" part of the B200-first design.
+"CUDA graphs instead of a tracing compiler" part of the design.
 """
 from __future__ import annotations
 

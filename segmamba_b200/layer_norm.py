@@ -15,7 +15,7 @@ from torch.amp import custom_bwd, custom_fwd
 
 from . import _lib
 
-# Default on (hardware parity: tests/test_gpu_layernorm.py; step 98.4 -> 94.7 ms, profiles/r2a_bench_ab.md);
+# Default on (hardware parity: tests/test_gpu_layernorm.py);
 # SMB_FUSED_LAYERNORM=0 keeps nn.LayerNorm for A/B runs.
 ENABLED = os.environ.get("SMB_FUSED_LAYERNORM", "1") != "0"
 

@@ -3,8 +3,8 @@
 ``cat_channels(a, b)`` == ``torch.cat((a, b), dim=1)`` for 5-D tensors stored channels-last (NDHWC): the (tokens, C) matrices of the two
 operands are copied into the left / right column block of the (tokens, Ca + Cb) result with full 16-byte vectors; the backward copies the
 two column blocks of the incoming gradient back out.  Replaces ``torch.cat((out, skip), dim=1)`` of UnetrUpBlock
-(monai/networks/blocks/unetr_block.py:81-86), which ATen runs as generic strided elementwise copies (2 x 0.44 ms forward and 2 x 0.44 ms
-backward per step at decoder2 alone).  Operands that do not meet the layout / alignment rules raise; the caller decides (segmamba.py
+(monai/networks/blocks/unetr_block.py:81-86), which ATen runs as generic strided elementwise copies (two forward and two
+backward per up block and step).  Operands that do not meet the layout / alignment rules raise; the caller decides (segmamba.py
 uses torch.cat for them).
 """
 from __future__ import annotations

@@ -144,7 +144,7 @@ class Mamba(nn.Module):
 
         if DIRECTION_STREAMS and xz.is_cuda:
             # The three directional passes are independent until the sum below.  At the deep stages (L = 4096 / 512) one pass
-            # cannot fill 148 SMs, so the reversed and the inter-slice pass are enqueued on two side streams (forked from and
+            # cannot fill 132 SMs, so the reversed and the inter-slice pass are enqueued on two side streams (forked from and
             # joined to the caller's stream; inside a CUDA-graph capture these become parallel branches).  Autograd replays
             # each branch's backward on the stream its forward ran on.  Opt-in until measured (SMB_DIR_STREAMS=1).
             cur = torch.cuda.current_stream()

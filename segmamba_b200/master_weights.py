@@ -2,7 +2,7 @@
 
 Under ``torch.autocast`` every convolution / linear weight is cast fp32 -> bf16 at its first use of each forward and its bf16
 gradient is cast back to fp32 in the backward: for the default SegMamba that is ~400 tiny cast kernels per training step
-(172 + 175 + 48 launches, 2.5 ms of the 101.9 ms step, profiles/r1_launches_train_step_v3.csv).  ``MasterWeights`` keeps the
+(172 + 175 + 48 launches).  ``MasterWeights`` keeps the
 arithmetic and removes the launches: the matmul / convolution parameters of the model are stored in bf16 (exactly the values the
 autocast cast would produce, so the forward and backward are bit-identical), the optimizer owns fp32 masters, and the two
 directions of the copy are one multi-tensor op each per step:

@@ -120,7 +120,7 @@ def fwd(u, delta, A, B, C, D_, z_, delta_bias_, delta_softplus):
     return [out, x, out_z] if z_ is not None else [out, x]
 
 
-LOW_MEMORY_BWD = True      # True: chunk-parallel recompute backward (small workspace; currently the faster one on B200);
+LOW_MEMORY_BWD = True      # True: chunk-parallel recompute backward (small workspace; the default);
                            # False: state-stash forward-recompute + lane-per-channel reverse sweep (workspace = B*L*N*D elements)
 
 

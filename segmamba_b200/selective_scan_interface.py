@@ -168,8 +168,7 @@ class MambaInnerFnNoOutProj(torch.autograd.Function):
         # views of their result -- no 'b d l -> (b l) d' transpose copy (ssi.py:181) and no .contiguous() of B / C (:187-207).
         conv2 = _as_dbl(conv1d_out)                                                     # (d_inner, b*l)
         # dt_rank = ceil(d_model / 16) is 3 / 6 / 12 at the first three stages: GEMMs with a 3- or 6-element leading dimension
-        # fall back to cuBLAS's unaligned legacy kernels (cutlass_75_*_align1 in profiles/r1_launches_train_step_v3.csv, up to
-        # 0.26 ms for a 96 x 3 output).  The two small weights are therefore zero-padded so that the dt block of x_dbl has R8 =
+        # fall back to cuBLAS's unaligned legacy kernels (cutlass_75_*_align1).  The two small weights are therefore zero-padded so that the dt block of x_dbl has R8 =
         # 8 / 8 / 16 rows and B, C start on 8-row boundaries; the padding rows / columns are exact zeros everywhere.
         R8 = -(-delta_rank // 8) * 8 if ALIGN_GEMMS else delta_rank
         if R8 != delta_rank:

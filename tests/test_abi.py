@@ -2,6 +2,7 @@
 the ctypes structures match the header's field lists, and the product fails loudly without a GPU / library."""
 import os
 import re
+import shutil
 import subprocess
 
 import pytest
@@ -58,13 +59,14 @@ def test_ctypes_structs_match_header(cname, pyname):
     assert py == _header_struct_fields(cname)
 
 
-def test_sm100a_tma_free_sass_present():
-    """the library carries sm_100a SASS (cuobjdump lists the arch) -- built for B200, not a generic PTX blob."""
+def test_sm90a_sass_present():
+    """the library carries sm_90a SASS (cuobjdump lists the arch) -- built for H100, not a generic PTX blob."""
     from segmamba_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         pytest.skip("library not built")
-    out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    out = subprocess.run([cuobjdump, "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in out
 
 
 def test_no_cpu_fallback():

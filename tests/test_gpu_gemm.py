@@ -1,4 +1,4 @@
-"""Tensor-core GEMM (smb_gemm: TMA + tcgen05.mma + tensor memory) against a plain fp32 torch product of the same 16-bit
+"""Tensor-core GEMM (smb_gemm: TMA + wgmma) against a plain fp32 torch product of the same 16-bit
 operands, at the shapes of the model's pointwise contractions (SURVEY.md section 8d) and at ragged ones; every operand-major
 combination, every epilogue, split-K accumulation, and the autograd wrapper ``gemm.linear`` against F.linear."""
 import pytest

@@ -23,7 +23,7 @@ def test_gemm_operand_major_detection():
 def test_gemm_routing_and_split_k():
     from segmamba_b200 import gemm as G
     assert G.MODE in ("auto", "all", "off") and G.SPLIT_TOKENS == 16384
-    assert G._split_k_for(524288) == 148 and G._split_k_for(65536) == 128 and G._split_k_for(1000) == 1
+    assert G._split_k_for(524288) == 132 and G._split_k_for(65536) == 128 and G._split_k_for(1000) == 1
 
 
 def test_gemm_and_layout_raise_on_cpu_tensors():

@@ -34,7 +34,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--stages", default="0,1,2,3")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "gemm_bench.json"))
+    ap.add_argument("--out", default=os.path.join(ROOT, "bench_out", "gemm_bench.json"))
     args = ap.parse_args()
     from segmamba_b200 import gemm as G
     dev, bf = "cuda", torch.bfloat16

@@ -24,6 +24,6 @@ for name, a, b in cases:
     c = prof.tolist()
     M, K = a.shape; N = b.shape[0]
     tiles = ((M + 127) // 128) * ((N + 255) // 256 if N > 256 else 1)
-    print(f"{name}: {s.elapsed_time(e)*1e3:.1f} us; per-CTA kcycles (148 CTAs): total {c[7]/148e3:.1f}  producer-wait-empty {c[0]/148e3:.1f}  "
-          f"mma-wait-tempty {c[1]/148e3:.1f}  mma-wait-full {c[2]/148e3:.1f}  epi-wait-tfull {[round(x/148e3,1) for x in c[3:7]]}  tiles {tiles}\n"
-          f"      epilogue warp 2 per CTA kcycles: tile total {c[11]/148e3:.1f} = wait::ld {c[8]/148e3:.1f} + copy-out {c[10]/148e3:.1f} + convert/stage {(c[11]-c[8]-c[10])/148e3:.1f}")
+    ctas = min(tiles, torch.cuda.get_device_properties(0).multi_processor_count) * 1e3
+    print(f"{name}: {s.elapsed_time(e)*1e3:.1f} us; per-CTA kcycles ({ctas / 1e3:.0f} CTAs): first consumer warp total {c[7]/ctas:.1f}  "
+          f"producer-wait-empty {c[0]/ctas:.1f}  consumer-wait-full {c[2]/ctas:.1f}  epilogue {c[11]/ctas:.1f}  tiles {tiles}")

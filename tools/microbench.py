@@ -1,8 +1,8 @@
-"""Op-level timing on B200: native scan / conv1d vs the REFERENCE's own CUDA kernels (oracle/_ref, compiled for sm_100a).
+"""Op-level timing on H100: native scan / conv1d vs the REFERENCE's own CUDA kernels (oracle/_ref, compiled for sm_90a).
 
 Measurement tool (not product, not a bench.py value).  CUDA events on the launching stream, >= 3 warm-ups, L2 flushed
 between iterations by writing a 512 MB buffer.  Also cross-checks the two implementations against each other (the
-reference extension is a second, GPU-side oracle).  Writes gpurun_out/microbench.json and a markdown table.
+reference extension is a second, GPU-side oracle).  Writes bench_out/microbench.json and a markdown table.
 
     python tools/microbench.py [--iters 10] [--dtypes f32,bf16] [--batches 1,2]
 """
@@ -56,7 +56,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--dtypes", default="f32,bf16")
     ap.add_argument("--batches", default="1,2")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "microbench.json"))
+    ap.add_argument("--out", default=os.path.join(ROOT, "bench_out", "microbench.json"))
     ap.add_argument("--stages", default="0,1,2,3")
     ap.add_argument("--no-ref", action="store_true")
     ap.add_argument("--no-dense", action="store_true", help="A/B: 256-position checkpoints only (warp-scan main backward pass)")
@@ -70,7 +70,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))     # H100 SXM data sheet unless a measured peak is given
     dev = "cuda"
     flush = torch.empty(128 * 1024 * 1024, device=dev)
     rows = []

@@ -32,7 +32,7 @@ def main():
         for _ in range(3):
             step()
         durs = prof.durations()
-    hbm = 6479.6
+    hbm = 3350.0     # H100 SXM data sheet, GB/s
     rows = []
     for (op, meta), d in durs.items():
         ms = sum(d) / 3

@@ -1,8 +1,8 @@
 """Run ONE training step (or one op set) inside a cudaProfilerStart/Stop range, for ncu --profile-from-start off.
 
-    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
+    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file bench_out/launches.csv \
         python tools/profile_step.py --what step
-    ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:scan_ -o gpurun_out/scan_full \
+    ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:scan_ -o bench_out/scan_full \
         python tools/profile_step.py --what scan
 """
 import argparse

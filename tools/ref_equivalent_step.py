@@ -1,8 +1,8 @@
 """Training step with the REFERENCE's op sequence on the reference's own CUDA kernels -- the denominator of the
 "x times the reference CUDA path" target (BASELINE.md section 3a).  Measurement tool, not product, not a bench.py value.
 
-/root/reference does not travel to the GPU box, so the reference model cannot be imported there.  What does travel:
-  * oracle/_ref/{selective_scan_cuda,causal_conv1d_cuda}.so -- the reference's kernels, compiled for sm_100a from its sources
+The reference checkout is not needed at run time, so the reference model is not imported.  What is used instead:
+  * oracle/_ref/{selective_scan_cuda,causal_conv1d_cuda}.so -- the reference's kernels, compiled for sm_90a from its sources
     (oracle/build_ref.py);
   * oracle/oracle.py -- the restatement of the reference's Python (SegMamba.forward, Mamba.forward v3,
     MambaInnerFnNoOutProj.forward with its flips / stack / rearrange copies, NCDHW layout, ATen InstanceNorm3d / LayerNorm),
@@ -30,7 +30,7 @@ sys.path.insert(0, ROOT)
 def load_ref(name):
     path = os.path.join(ROOT, "oracle", "_ref", name + ".so")
     if not os.path.exists(path):
-        raise SystemExit(f"{path} is missing: run `python oracle/build_ref.py` in the build container first")
+        raise SystemExit(f"{path} is missing: run `python oracle/build_ref.py` where the reference checkout is present first")
     spec = importlib.util.spec_from_file_location(name, path)
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
@@ -119,7 +119,7 @@ def main():
     ap.add_argument("--patch", type=int, default=128)
     ap.add_argument("--native", action="store_true", help="also time the native module on the same inputs")
     ap.add_argument("--dry-run-cpu", action="store_true", help="plumbing check without a GPU: tiny model, CPU oracle kernels")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "ref_equivalent_step.json"))
+    ap.add_argument("--out", default=os.path.join(ROOT, "bench_out", "ref_equivalent_step.json"))
     args = ap.parse_args()
     from oracle import oracle as orc
     from segmamba_b200.segmamba import SegMamba

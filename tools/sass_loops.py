@@ -2,7 +2,7 @@
 
 usage: python tools/sass_loops.py <lib.so> <mangled-kernel-substring> [min_len]
 For every backward branch (loop) prints the body length and the opcode histogram, so the instructions per scan update can
-be counted before spending GPU time (B200_PROFILING.md: check SASS here first).
+be counted before spending GPU time.
 """
 import collections
 import re

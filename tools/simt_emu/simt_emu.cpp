@@ -375,7 +375,7 @@ void run_grid(const std::function<void()> &body, dim3 grid, dim3 block, size_t s
         abort();
     }
     if (smem_bytes > 227 * 1024) {
-        fprintf(stderr, "simt_emu: %zu bytes of dynamic shared memory exceed the 227 KB of an sm_100 CTA\n", smem_bytes);
+        fprintf(stderr, "simt_emu: %zu bytes of dynamic shared memory exceed the 227 KB of an sm_90 CTA\n", smem_bytes);
         abort();
     }
     std::atomic<long> next{0};

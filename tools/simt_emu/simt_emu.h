@@ -226,9 +226,6 @@ inline int __float_as_int(float f) { int i; std::memcpy(&i, &f, 4); return i; }
 inline float __int_as_float(int i) { float f; std::memcpy(&f, &i, 4); return f; }
 inline unsigned __float_as_uint(float f) { unsigned i; std::memcpy(&i, &f, 4); return i; }
 inline float __uint_as_float(unsigned i) { float f; std::memcpy(&f, &i, 4); return f; }
-inline float2 __ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(std::fma(a.x, b.x, c.x), std::fma(a.y, b.y, c.y)); }
-inline float2 __fmul2_rn(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
-inline float2 __fadd2_rn(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 template <typename T> inline T __ldg(const T *p) { return *p; }
 inline int min(int a, int b) { return a < b ? a : b; }
 inline int max(int a, int b) { return a > b ? a : b; }
