@@ -313,6 +313,138 @@ SMB_API int smb_gemm(const smb_gemm_args *args, void *cuda_stream);
 SMB_API int smb_copy2d(const void *src, int64_t src_pitch_bytes, void *dst, int64_t dst_pitch_bytes, int64_t rows, int64_t row_bytes,
                        void *cuda_stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Training-patch sampling and augmentation on the GPU (segmamba_b200/augment.py, patch_loader.py): the crop of
+ * DataLoaderMultiProcess (light_training/dataloading/base_data_loader.py:39-213) and the transforms of get_train_transforms
+ * (light_training/augment/train_augment.py:23-62), as stages the host composes.  Every random draw is made by the host and
+ * arrives here as a parameter; the only randomness on the device is the Gaussian noise of smb_aug_pointwise, a counter-based
+ * Philox4x32-10 stream keyed by the 64-bit seed, counter (voxel / 4, step, sample, channel), so every value can be recomputed.
+ * Volumes are (n0, n1, n2) fp32 with axis 2 contiguous.  Job lists are host arrays of any length; the records are copied into
+ * the kernel parameters, so the array may be reused as soon as the call returns.  Kernels are enqueued on `cuda_stream`; no
+ * allocation and no host synchronisation happen inside.  Volume axes are limited to 4..256 samples.
+ * ---------------------------------------------------------------------------------------------- */
+enum { SMB_AUG_MIRROR = 0, SMB_AUG_EDGE = 1 };        /* spline boundary: scipy 'mirror' / 'nearest' */
+enum { SMB_AUG_AFFINE = 0, SMB_AUG_ZOOM = 1 };        /* resample coordinate map */
+enum { SMB_AUG_OP_RETAIN = 1, SMB_AUG_OP_UNINVERT = 2, SMB_AUG_OP_NOISE = 4, SMB_AUG_OP_BRIGHT = 8, SMB_AUG_OP_CONTRAST = 16,
+       SMB_AUG_OP_INVERT = 32, SMB_AUG_OP_GAMMA = 64 };
+#define SMB_AUG_STATS_SCRATCH 512                      /* doubles of scratch per stats job */
+
+/* crop box of one sample: out[c, i, j, k] = data[c, lz + i, ly + j, lx + k] inside the case, 0 outside (seg likewise) */
+typedef struct smb_aug_case {
+    const float *data;          /* (channels, D, H, W) fp32, W contiguous: device memory, or page-locked host memory read
+                                   through its device mapping (then only the crop box crosses the bus) */
+    const void *seg;            /* (D, H, W) int8, W contiguous, same placement rules */
+    int64_t data_cs, data_zs, data_ys;
+    int64_t seg_zs, seg_ys;
+    int32_t D, H, W;
+    int32_t lz, ly, lx;
+} smb_aug_case;
+
+typedef struct smb_aug_crop_args {
+    int32_t batch, channels, pd, ph, pw;
+    const smb_aug_case *cases;  /* `batch` records (host array) */
+    float *data;                /* (batch, channels, pd, ph, pw) fp32 */
+    void *seg;                  /* (batch, pd, ph, pw) int8 */
+} smb_aug_crop_args;
+
+SMB_API int smb_aug_crop(const smb_aug_crop_args *args, void *cuda_stream);
+
+/* cubic B-spline coefficients of src (scipy.ndimage.spline_filter, order 3) on a grid with a 2-sample border per side:
+ * coef is (n0 + 4, n1 + 4, n2 + 4).  SMB_AUG_MIRROR: whole-sample mirror boundary, the border holds the mirrored coefficients
+ * (map_coordinates mode 'constant' / 'mirror');  SMB_AUG_EDGE: the coefficients of src padded by 12 edge samples per side and
+ * filtered with the 'nearest' boundary, as scipy does for mode 'nearest' (zoom of skimage's resize, mode 'edge'). */
+typedef struct smb_aug_prefilter_job {
+    const float *src;           /* (n0, n1, n2) */
+    float *coef;                /* (n0 + 4, n1 + 4, n2 + 4); must not overlap src */
+    int32_t n0, n1, n2;
+    int32_t boundary;           /* SMB_AUG_MIRROR / SMB_AUG_EDGE */
+} smb_aug_prefilter_job;
+
+SMB_API int smb_aug_prefilter(const smb_aug_prefilter_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* dst[o] = src sampled at coordinate x(o), per axis d:
+ *   SMB_AUG_AFFINE  x_d = a_d0 o_0 + a_d1 o_1 + a_d2 o_2 + a_d3   (double); outside [0, n_d - 1] on any axis -> 0 / label 0
+ *   SMB_AUG_ZOOM    x_d = (o_d + 0.5) a_dd - 0.5                   (double; scipy zoom grid_mode, 'nearest' boundary)
+ * order 0: nearest sample, index floor(x + 0.5), src fp32 (n0, n1, n2);
+ * order 3: cubic B-spline, src the coef of smb_aug_prefilter;
+ * order 1: labels, src and dst int8: the label whose trilinearly interpolated indicator is largest and >= 0.5, else 0
+ *          (batchgenerators' interpolate_img(is_seg=True) with cval -1).
+ * clip (optional): a stats record of smb_aug_stats; data results are clipped to its [min, max]. */
+typedef struct smb_aug_resample_job {
+    const void *src;
+    void *dst;                  /* (m0, m1, m2) */
+    const double *clip;
+    int32_t n0, n1, n2, m0, m1, m2;
+    int32_t order;              /* 0, 1, 3 */
+    int32_t map;                /* SMB_AUG_AFFINE / SMB_AUG_ZOOM */
+    double a00, a01, a02, a03, a10, a11, a12, a13, a20, a21, a22, a23;
+} smb_aug_resample_job;
+
+SMB_API int smb_aug_resample(const smb_aug_resample_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* x <- scipy.ndimage.gaussian_filter(x, sigma, mode='reflect', truncate=4.0): three 1-D passes x -> tmp -> tmp + n -> x */
+typedef struct smb_aug_blur_job {
+    float *x;
+    float *tmp;                 /* 2 * n0 * n1 * n2 floats */
+    float sigma;
+    int32_t n0, n1, n2;
+} smb_aug_blur_job;
+
+SMB_API int smb_aug_blur(const smb_aug_blur_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* stats[0..3] = sum, sum of squares (fp64), min, max of x[0 .. n) */
+typedef struct smb_aug_stats_job {
+    const float *x;
+    double *stats;
+    double *scratch;            /* SMB_AUG_STATS_SCRATCH doubles */
+    int64_t n;
+} smb_aug_stats_job;
+
+SMB_API int smb_aug_stats(const smb_aug_stats_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* in-place pointwise chain over x[0 .. n), in this order, each step only when its bit is set in `ops`; mean, std, min, max
+ * come from `stats` (the state of x on entry), carried through the linear steps (brightness, inversion):
+ *   RETAIN    x = (x - mean) / (std + 1e-8) * sd_r + mn_r, with mn_r, sd_r the mean and std of `retain_ref`
+ *             (mn_r negated under UNINVERT: the reference was taken before the inversion of the gamma pass)
+ *   UNINVERT  x = -x
+ *   NOISE     x += noise_std * N(0, 1), Box-Muller on the Philox stream of (seed, step, sample, channel)
+ *   BRIGHT    x *= brightness
+ *   CONTRAST  x = clip((x - mean) * contrast + mean, min, max)
+ *   INVERT    x = -x
+ *   GAMMA     x = ((x - min) / (max - min + 1e-7)) ^ gamma * (max - min) + min
+ * A step that reads the statistics must not follow NOISE, CONTRAST or GAMMA in the same job. */
+typedef struct smb_aug_point_job {
+    float *x;
+    const double *stats;
+    const double *retain_ref;
+    int64_t n;
+    int64_t seed;
+    int32_t step, sample, channel;
+    int32_t ops;
+    float noise_std, brightness, contrast, gamma;
+} smb_aug_point_job;
+
+SMB_API int smb_aug_pointwise(const smb_aug_point_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* final layout: image[b, c, i, j, k] (or channels-last [b, i, j, k, c]) = data[c, f(i), f(j), f(k)] in out_dtype, label[b, i, j, k] =
+ * int64 of seg[f(i), f(j), f(k)] with -1 -> 0, where f mirrors an axis when its bit (1: axis 0, 2: axis 1, 4: axis 2) is set in flip */
+typedef struct smb_aug_emit_sample {
+    const float *data;          /* (channels, pd, ph, pw) */
+    const void *seg;            /* (pd, ph, pw) int8 */
+    int32_t flip;
+} smb_aug_emit_sample;
+
+typedef struct smb_aug_emit_args {
+    int32_t batch, channels, pd, ph, pw;
+    int32_t out_dtype;          /* SMB_F32 / SMB_F16 / SMB_BF16 */
+    int32_t channels_last;
+    const smb_aug_emit_sample *samples;   /* `batch` records (host array) */
+    void *image;
+    int64_t *label;
+} smb_aug_emit_args;
+
+SMB_API int smb_aug_emit(const smb_aug_emit_args *args, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

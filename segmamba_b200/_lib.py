@@ -102,6 +102,59 @@ class GemmArgs(ctypes.Structure):
                 + [(n, _vp) for n in ("A", "B", "bias", "D")] + [(n, _i64) for n in ("lda", "ldb", "ldd")])
 
 
+# training-patch augmentation (include/segmamba_b200.h, "Training-patch sampling and augmentation")
+_f64, _f32 = ctypes.c_double, ctypes.c_float
+
+
+class AugCase(ctypes.Structure):
+    _fields_ = ([("data", _vp), ("seg", _vp)] + [(n, _i64) for n in ("data_cs", "data_zs", "data_ys", "seg_zs", "seg_ys")]
+                + [(n, _i32) for n in ("D", "H", "W", "lz", "ly", "lx")])
+
+
+class AugCropArgs(ctypes.Structure):
+    _fields_ = ([(n, _i32) for n in ("batch", "channels", "pd", "ph", "pw")]
+                + [("cases", ctypes.POINTER(AugCase)), ("data", _vp), ("seg", _vp)])
+
+
+class AugPrefilterJob(ctypes.Structure):
+    _fields_ = [("src", _vp), ("coef", _vp)] + [(n, _i32) for n in ("n0", "n1", "n2", "boundary")]
+
+
+class AugResampleJob(ctypes.Structure):
+    _fields_ = ([("src", _vp), ("dst", _vp), ("clip", _vp)]
+                + [(n, _i32) for n in ("n0", "n1", "n2", "m0", "m1", "m2", "order", "map")]
+                + [(f"a{r}{c}", _f64) for r in range(3) for c in range(4)])
+
+
+class AugBlurJob(ctypes.Structure):
+    _fields_ = [("x", _vp), ("tmp", _vp), ("sigma", _f32)] + [(n, _i32) for n in ("n0", "n1", "n2")]
+
+
+class AugStatsJob(ctypes.Structure):
+    _fields_ = [("x", _vp), ("stats", _vp), ("scratch", _vp), ("n", _i64)]
+
+
+class AugPointJob(ctypes.Structure):
+    _fields_ = ([("x", _vp), ("stats", _vp), ("retain_ref", _vp), ("n", _i64), ("seed", _i64)]
+                + [(n, _i32) for n in ("step", "sample", "channel", "ops")]
+                + [(n, _f32) for n in ("noise_std", "brightness", "contrast", "gamma")])
+
+
+class AugEmitSample(ctypes.Structure):
+    _fields_ = [("data", _vp), ("seg", _vp), ("flip", _i32)]
+
+
+class AugEmitArgs(ctypes.Structure):
+    _fields_ = ([(n, _i32) for n in ("batch", "channels", "pd", "ph", "pw", "out_dtype", "channels_last")]
+                + [("samples", ctypes.POINTER(AugEmitSample)), ("image", _vp), ("label", _vp)])
+
+
+AUG_MIRROR, AUG_EDGE = 0, 1
+AUG_AFFINE, AUG_ZOOM = 0, 1
+(OP_RETAIN, OP_UNINVERT, OP_NOISE, OP_BRIGHT, OP_CONTRAST, OP_INVERT, OP_GAMMA) = (1, 2, 4, 8, 16, 32, 64)
+AUG_STATS_SCRATCH = 512
+
+
 # every symbol include/segmamba_b200.h declares (tests/test_abi.py checks the header against this list)
 EXPORTS = {
     "smb_version": (ctypes.c_int, []),
@@ -122,6 +175,13 @@ EXPORTS = {
     "smb_layernorm_bwd": (ctypes.c_int, [ctypes.POINTER(LayerNormBwdArgs), _vp]),
     "smb_gemm": (ctypes.c_int, [ctypes.POINTER(GemmArgs), _vp]),
     "smb_copy2d": (ctypes.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _vp]),
+    "smb_aug_crop": (ctypes.c_int, [ctypes.POINTER(AugCropArgs), _vp]),
+    "smb_aug_prefilter": (ctypes.c_int, [ctypes.POINTER(AugPrefilterJob), _i32, _vp]),
+    "smb_aug_resample": (ctypes.c_int, [ctypes.POINTER(AugResampleJob), _i32, _vp]),
+    "smb_aug_blur": (ctypes.c_int, [ctypes.POINTER(AugBlurJob), _i32, _vp]),
+    "smb_aug_stats": (ctypes.c_int, [ctypes.POINTER(AugStatsJob), _i32, _vp]),
+    "smb_aug_pointwise": (ctypes.c_int, [ctypes.POINTER(AugPointJob), _i32, _vp]),
+    "smb_aug_emit": (ctypes.c_int, [ctypes.POINTER(AugEmitArgs), _vp]),
 }
 
 _lib = None

@@ -6,6 +6,7 @@
 #include <cstring>
 
 #include "../../include/segmamba_b200.h"
+#include "aug_internal.h"
 #include "conv_internal.h"
 #include "gemm_internal.h"
 #include "norm_internal.h"
@@ -427,6 +428,108 @@ SMB_API int smb_copy2d(const void *src, int64_t src_pitch_bytes, void *dst, int6
     if (rows == 0) return SMB_OK;
     cudaError_t e = smb::copy2d_launch(src, src_pitch_bytes, dst, dst_pitch_bytes, rows, row_bytes, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_copy2d");
+    return SMB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// training-patch augmentation (augment.cu)
+static bool aug_axis_ok(int n) { return n >= 1 && n <= smb::kAugMaxAxis; }
+
+SMB_API int smb_aug_crop(const smb_aug_crop_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_aug_crop: null args");
+    if (a->batch <= 0 || a->channels <= 0 || !aug_axis_ok(a->pd) || !aug_axis_ok(a->ph) || !aug_axis_ok(a->pw))
+        return fail(SMB_EINVAL, "smb_aug_crop: batch, channels must be positive and patch axes in 1..%d", smb::kAugMaxAxis);
+    if (!a->cases || !a->data || !a->seg) return fail(SMB_EINVAL, "smb_aug_crop: cases, data, seg are required");
+    for (int s = 0; s < a->batch; ++s) {
+        const smb_aug_case &c = a->cases[s];
+        if (!c.data || !c.seg || c.D <= 0 || c.H <= 0 || c.W <= 0) return fail(SMB_EINVAL, "smb_aug_crop: case %d has no data / seg or an empty shape", s);
+    }
+    cudaError_t e = smb::aug_crop_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_crop");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_prefilter(const smb_aug_prefilter_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_aug_prefilter: bad job list");
+    for (int q = 0; q < n_jobs; ++q) {
+        const smb_aug_prefilter_job &j = jobs[q];
+        if (!j.src || !j.coef) return fail(SMB_EINVAL, "smb_aug_prefilter: job %d needs src and coef", q);
+        if (j.n0 < 4 || j.n1 < 4 || j.n2 < 4 || j.n0 > smb::kAugMaxAxis || j.n1 > smb::kAugMaxAxis || j.n2 > smb::kAugMaxAxis)
+            return fail(SMB_EUNSUPPORTED, "smb_aug_prefilter: job %d: axes must be 4..%d samples", q, smb::kAugMaxAxis);
+        if (j.boundary != SMB_AUG_MIRROR && j.boundary != SMB_AUG_EDGE) return fail(SMB_EINVAL, "smb_aug_prefilter: job %d: bad boundary", q);
+    }
+    cudaError_t e = smb::aug_prefilter_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_prefilter");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_resample(const smb_aug_resample_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_aug_resample: bad job list");
+    for (int q = 0; q < n_jobs; ++q) {
+        const smb_aug_resample_job &j = jobs[q];
+        if (!j.src || !j.dst) return fail(SMB_EINVAL, "smb_aug_resample: job %d needs src and dst", q);
+        if (!aug_axis_ok(j.n0) || !aug_axis_ok(j.n1) || !aug_axis_ok(j.n2) || !aug_axis_ok(j.m0) || !aug_axis_ok(j.m1) || !aug_axis_ok(j.m2))
+            return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: axes must be 1..%d samples", q, smb::kAugMaxAxis);
+        if (j.order != 0 && j.order != 1 && j.order != 3) return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: order %d (0, 1, 3)", q, j.order);
+        if (j.map != SMB_AUG_AFFINE && j.map != SMB_AUG_ZOOM) return fail(SMB_EINVAL, "smb_aug_resample: job %d: bad map", q);
+        if (j.order == 1 && (j.map != SMB_AUG_AFFINE || j.clip)) return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: labels take an affine map, no clip", q);
+    }
+    cudaError_t e = smb::aug_resample_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_resample");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_blur(const smb_aug_blur_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_aug_blur: bad job list");
+    for (int q = 0; q < n_jobs; ++q) {
+        const smb_aug_blur_job &j = jobs[q];
+        if (!j.x || !j.tmp) return fail(SMB_EINVAL, "smb_aug_blur: job %d needs x and tmp", q);
+        if (!aug_axis_ok(j.n0) || !aug_axis_ok(j.n1) || !aug_axis_ok(j.n2)) return fail(SMB_EUNSUPPORTED, "smb_aug_blur: job %d: bad shape", q);
+        if (!(j.sigma > 0.f && j.sigma <= 2.f)) return fail(SMB_EUNSUPPORTED, "smb_aug_blur: job %d: sigma must be in (0, 2]", q);
+    }
+    cudaError_t e = smb::aug_blur_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_blur");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_stats(const smb_aug_stats_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_aug_stats: bad job list");
+    for (int q = 0; q < n_jobs; ++q)
+        if (!jobs[q].x || !jobs[q].stats || !jobs[q].scratch || jobs[q].n <= 0) return fail(SMB_EINVAL, "smb_aug_stats: job %d: x, stats, scratch, n > 0 required", q);
+    cudaError_t e = smb::aug_stats_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_stats");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_pointwise(const smb_aug_point_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_aug_pointwise: bad job list");
+    for (int q = 0; q < n_jobs; ++q) {
+        const smb_aug_point_job &j = jobs[q];
+        if (!j.x || j.n <= 0) return fail(SMB_EINVAL, "smb_aug_pointwise: job %d: x and n > 0 required", q);
+        if ((j.ops & ~127) != 0) return fail(SMB_EINVAL, "smb_aug_pointwise: job %d: unknown op bits", q);
+        if ((j.ops & (SMB_AUG_OP_RETAIN | SMB_AUG_OP_CONTRAST | SMB_AUG_OP_GAMMA)) && !j.stats)
+            return fail(SMB_EINVAL, "smb_aug_pointwise: job %d: retain / contrast / gamma need stats", q);
+        if ((j.ops & SMB_AUG_OP_RETAIN) && !j.retain_ref) return fail(SMB_EINVAL, "smb_aug_pointwise: job %d: retain needs retain_ref", q);
+        const int nonlinear_before_stats =
+            ((j.ops & SMB_AUG_OP_NOISE) && (j.ops & (SMB_AUG_OP_CONTRAST | SMB_AUG_OP_GAMMA))) ||
+            ((j.ops & SMB_AUG_OP_CONTRAST) && (j.ops & SMB_AUG_OP_GAMMA));
+        if (nonlinear_before_stats) return fail(SMB_EINVAL, "smb_aug_pointwise: job %d: a statistics-driven step follows a nonlinear one", q);
+    }
+    cudaError_t e = smb::aug_pointwise_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_pointwise");
+    return SMB_OK;
+}
+
+SMB_API int smb_aug_emit(const smb_aug_emit_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_aug_emit: null args");
+    if (a->batch <= 0 || a->channels <= 0 || !aug_axis_ok(a->pd) || !aug_axis_ok(a->ph) || !aug_axis_ok(a->pw))
+        return fail(SMB_EINVAL, "smb_aug_emit: bad shape");
+    if (a->out_dtype < SMB_F32 || a->out_dtype > SMB_BF16) return fail(SMB_EINVAL, "smb_aug_emit: bad out_dtype %d", a->out_dtype);
+    if (!a->samples || !a->image || !a->label) return fail(SMB_EINVAL, "smb_aug_emit: samples, image, label are required");
+    for (int s = 0; s < a->batch; ++s)
+        if (!a->samples[s].data || !a->samples[s].seg) return fail(SMB_EINVAL, "smb_aug_emit: sample %d needs data and seg", s);
+    cudaError_t e = smb::aug_emit_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_aug_emit");
     return SMB_OK;
 }
 
