@@ -445,6 +445,77 @@ typedef struct smb_aug_emit_args {
 
 SMB_API int smb_aug_emit(const smb_aug_emit_args *args, void *cuda_stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Segmentation metrics on the GPU (segmamba_b200/metrics.py): Dice and the Hausdorff percentile of medpy.metric.binary
+ * (dc, hd95, hd with connectivity 1) per (sample, region), from region bitmasks.  A region is a set of label values; voxel
+ * bit r is set when the voxel belongs to region r (up to 8 regions).  Volumes are (batch, d, h, w) with w contiguous.
+ * Stages, all on `cuda_stream`, with no allocation and no host synchronisation inside:
+ *   smb_metric_region_bits  labels or logits (argmax over classes, first maximum wins) -> bits
+ *   smb_metric_count        per (sample, region) counts and the two border masks (a foreground voxel with a 6-neighbour in
+ *                           the background or outside the volume)
+ *   smb_metric_edt          exact Euclidean distance from every border voxel of one mask to the nearest border voxel of the
+ *                           other, appended to the (sample, region) pool
+ *   smb_metric_select       the q-th percentile of each pool (numpy 'linear'), NaN where a mask is empty
+ * Every count is an integer atomic and every pool is reduced by an order-free radix select: results are bitwise
+ * deterministic.  Axes h and w are limited to 1..SMB_METRIC_MAX_AXIS voxels, d * h * w to 2^31 - 1.
+ * ---------------------------------------------------------------------------------------------- */
+#define SMB_METRIC_MAX_REGIONS 8
+#define SMB_METRIC_MAX_AXIS 768
+#define SMB_METRIC_NCOUNTS 8          /* int64 per (sample, region), see smb_metric_count */
+enum { SMB_METRIC_I8 = 0, SMB_METRIC_U8 = 1, SMB_METRIC_I32 = 2, SMB_METRIC_I64 = 3, SMB_METRIC_LOGITS = 4 };
+
+/* bits[b, v] = lut[label] for labels 0..255 (0 outside), label = src[b, v] or, for SMB_METRIC_LOGITS, argmax over
+ * c < classes of src[b * sample_stride + c * class_stride + v * voxel_stride] (dtype SMB_F32 / SMB_F16 / SMB_BF16; a NaN is
+ * the maximum, as in torch.argmax).  Labels are read at b * sample_stride + v * voxel_stride.  Strides in elements. */
+typedef struct smb_metric_bits_args {
+    const void *src;
+    void *bits;                 /* (batch, voxels) uint8 */
+    int64_t voxels, sample_stride, class_stride, voxel_stride;
+    int32_t batch, kind, dtype, classes;
+    uint8_t lut[256];
+} smb_metric_bits_args;
+
+SMB_API int smb_metric_region_bits(const smb_metric_bits_args *args, void *cuda_stream);
+
+/* counts[(b * regions + r) * SMB_METRIC_NCOUNTS + k] += |P|, |G|, |P and G|, |border P|, |border G| for k = 0..4 (k = 5 is
+ * the pool fill of smb_metric_edt; the caller zeroes counts first); the border masks get bit r of the border voxels. */
+typedef struct smb_metric_count_args {
+    const void *pred, *target;  /* (batch, d, h, w) uint8 region bits */
+    void *pred_border, *target_border;
+    int64_t *counts;
+    int32_t batch, regions, d, h, w;
+} smb_metric_count_args;
+
+SMB_API int smb_metric_count(const smb_metric_count_args *args, void *cuda_stream);
+
+/* For each (b, r, direction): the distance, with spacing s0, s1, s2 per axis, from every voxel of the source border (P's, then
+ * G's) to the nearest voxel of the other border, sqrt(((dz s0)^2 + (dy s1)^2) + (dx s2)^2) in fp64, appended at
+ * pool[(b * regions + r) * pool_cap + i] with i from the fill counter counts[.. + 5].  feat: batch * regions * 2 * d * h * w
+ * int32 of workspace.  pool_cap must be at least 2 * d * h * w. */
+typedef struct smb_metric_edt_args {
+    const void *pred_border, *target_border;
+    int32_t *feat;
+    double *pool;
+    int64_t *counts;
+    int64_t pool_cap;
+    int32_t batch, regions, d, h, w;
+    double s0, s1, s2;
+} smb_metric_edt_args;
+
+SMB_API int smb_metric_edt(const smb_metric_edt_args *args, void *cuda_stream);
+
+/* out[b, r] = numpy.percentile(pool of (b, r), 100 * frac) with method 'linear', NaN where |P| or |G| is 0 */
+typedef struct smb_metric_select_args {
+    const double *pool;
+    const int64_t *counts;
+    double *out;                /* (batch, regions) */
+    int64_t pool_cap;
+    int32_t batch, regions;
+    double frac;                /* q / 100, in [0, 1] */
+} smb_metric_select_args;
+
+SMB_API int smb_metric_select(const smb_metric_select_args *args, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

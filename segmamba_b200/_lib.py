@@ -155,6 +155,31 @@ AUG_AFFINE, AUG_ZOOM = 0, 1
 AUG_STATS_SCRATCH = 512
 
 
+# segmentation metrics (include/segmamba_b200.h, "Segmentation metrics on the GPU")
+class MetricBitsArgs(ctypes.Structure):
+    _fields_ = ([("src", _vp), ("bits", _vp)] + [(n, _i64) for n in ("voxels", "sample_stride", "class_stride", "voxel_stride")]
+                + [(n, _i32) for n in ("batch", "kind", "dtype", "classes")] + [("lut", ctypes.c_uint8 * 256)])
+
+
+class MetricCountArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("pred", "target", "pred_border", "target_border", "counts")]
+                + [(n, _i32) for n in ("batch", "regions", "d", "h", "w")])
+
+
+class MetricEdtArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("pred_border", "target_border", "feat", "pool", "counts")] + [("pool_cap", _i64)]
+                + [(n, _i32) for n in ("batch", "regions", "d", "h", "w")] + [(n, _f64) for n in ("s0", "s1", "s2")])
+
+
+class MetricSelectArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("pool", "counts", "out")] + [("pool_cap", _i64)]
+                + [(n, _i32) for n in ("batch", "regions")] + [("frac", _f64)])
+
+
+METRIC_MAX_REGIONS, METRIC_MAX_AXIS, METRIC_NCOUNTS = 8, 768, 8
+METRIC_I8, METRIC_U8, METRIC_I32, METRIC_I64, METRIC_LOGITS = 0, 1, 2, 3, 4
+
+
 # every symbol include/segmamba_b200.h declares (tests/test_abi.py checks the header against this list)
 EXPORTS = {
     "smb_version": (ctypes.c_int, []),
@@ -182,6 +207,10 @@ EXPORTS = {
     "smb_aug_stats": (ctypes.c_int, [ctypes.POINTER(AugStatsJob), _i32, _vp]),
     "smb_aug_pointwise": (ctypes.c_int, [ctypes.POINTER(AugPointJob), _i32, _vp]),
     "smb_aug_emit": (ctypes.c_int, [ctypes.POINTER(AugEmitArgs), _vp]),
+    "smb_metric_region_bits": (ctypes.c_int, [ctypes.POINTER(MetricBitsArgs), _vp]),
+    "smb_metric_count": (ctypes.c_int, [ctypes.POINTER(MetricCountArgs), _vp]),
+    "smb_metric_edt": (ctypes.c_int, [ctypes.POINTER(MetricEdtArgs), _vp]),
+    "smb_metric_select": (ctypes.c_int, [ctypes.POINTER(MetricSelectArgs), _vp]),
 }
 
 _lib = None

@@ -1,5 +1,6 @@
 // extern "C" entry points of libsegmamba_b200.so (see include/segmamba_b200.h).
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdint>
@@ -9,6 +10,7 @@
 #include "aug_internal.h"
 #include "conv_internal.h"
 #include "gemm_internal.h"
+#include "metrics_internal.h"
 #include "norm_internal.h"
 #include "scan_internal.h"
 
@@ -530,6 +532,67 @@ SMB_API int smb_aug_emit(const smb_aug_emit_args *a, void *cuda_stream) {
         if (!a->samples[s].data || !a->samples[s].seg) return fail(SMB_EINVAL, "smb_aug_emit: sample %d needs data and seg", s);
     cudaError_t e = smb::aug_emit_launch(*a, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_aug_emit");
+    return SMB_OK;
+}
+
+// segmentation metrics (metrics.cu)
+static int metric_shape(int batch, int regions, int d, int h, int w, const char *who) {
+    if (batch <= 0 || batch > 65535 || d <= 0 || h <= 0 || w <= 0) return fail(SMB_EINVAL, "%s: batch (1..65535) and axes must be positive", who);
+    if (regions <= 0 || regions > SMB_METRIC_MAX_REGIONS) return fail(SMB_EINVAL, "%s: regions must be 1..%d", who, SMB_METRIC_MAX_REGIONS);
+    if (h > SMB_METRIC_MAX_AXIS || w > SMB_METRIC_MAX_AXIS) return fail(SMB_EUNSUPPORTED, "%s: axes 1 and 2 are limited to %d voxels", who, SMB_METRIC_MAX_AXIS);
+    if ((int64_t)d * h * w > INT32_MAX) return fail(SMB_EUNSUPPORTED, "%s: volumes are limited to 2^31 - 1 voxels", who);
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_region_bits(const smb_metric_bits_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_region_bits: null args");
+    if (!a->src || !a->bits) return fail(SMB_EINVAL, "smb_metric_region_bits: src and bits are required");
+    if (a->batch <= 0 || a->batch > 65535 || a->voxels <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: batch (1..65535) and voxels must be positive");
+    if (a->sample_stride < 0 || a->voxel_stride <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: bad strides");
+    if (a->kind < SMB_METRIC_I8 || a->kind > SMB_METRIC_LOGITS) return fail(SMB_EINVAL, "smb_metric_region_bits: bad kind %d", a->kind);
+    if (a->kind == SMB_METRIC_LOGITS) {
+        if (a->dtype < SMB_F32 || a->dtype > SMB_BF16) return fail(SMB_EINVAL, "smb_metric_region_bits: bad dtype %d", a->dtype);
+        if (a->classes <= 0 || a->class_stride <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: logits need classes and class_stride > 0");
+    }
+    cudaError_t e = smb::metric_bits_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_region_bits");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_count(const smb_metric_count_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_count: null args");
+    int rc = metric_shape(a->batch, a->regions, a->d, a->h, a->w, "smb_metric_count");
+    if (rc != SMB_OK) return rc;
+    if (!a->pred || !a->target || !a->pred_border || !a->target_border || !a->counts)
+        return fail(SMB_EINVAL, "smb_metric_count: pred, target, pred_border, target_border, counts are required");
+    cudaError_t e = smb::metric_count_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_count");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_edt(const smb_metric_edt_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_edt: null args");
+    int rc = metric_shape(a->batch, a->regions, a->d, a->h, a->w, "smb_metric_edt");
+    if (rc != SMB_OK) return rc;
+    if (a->batch * a->regions * 2 > 65535) return fail(SMB_EUNSUPPORTED, "smb_metric_edt: batch * regions * 2 is limited to 65535");
+    if (!a->pred_border || !a->target_border || !a->feat || !a->pool || !a->counts)
+        return fail(SMB_EINVAL, "smb_metric_edt: pred_border, target_border, feat, pool, counts are required");
+    if (a->pool_cap < 2 * (int64_t)a->d * a->h * a->w) return fail(SMB_EWORKSPACE, "smb_metric_edt: pool_cap must be at least 2 * d * h * w");
+    if (!(a->s0 > 0.0 && a->s1 > 0.0 && a->s2 > 0.0) || !std::isfinite(a->s0 * a->s1 * a->s2))
+        return fail(SMB_EINVAL, "smb_metric_edt: spacing must be positive and finite");
+    cudaError_t e = smb::metric_edt_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_edt");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_select(const smb_metric_select_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_select: null args");
+    if (!a->pool || !a->counts || !a->out) return fail(SMB_EINVAL, "smb_metric_select: pool, counts, out are required");
+    if (a->batch <= 0 || a->regions <= 0 || a->regions > SMB_METRIC_MAX_REGIONS || a->pool_cap <= 0 || (int64_t)a->batch * a->regions > INT32_MAX)
+        return fail(SMB_EINVAL, "smb_metric_select: bad batch / regions / pool_cap");
+    if (!(a->frac >= 0.0 && a->frac <= 1.0)) return fail(SMB_EINVAL, "smb_metric_select: frac must be in [0, 1]");
+    cudaError_t e = smb::metric_select_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_select");
     return SMB_OK;
 }
 

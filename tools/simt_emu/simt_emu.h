@@ -221,6 +221,9 @@ inline float __frsqrt_rn(float a) { return 1.f / std::sqrt(a); }
 inline float __fmaf_rn(float a, float b, float c) { return std::fma(a, b, c); }
 inline float __fmul_rn(float a, float b) { return a * b; }
 inline float __fadd_rn(float a, float b) { return a + b; }
+inline double __dmul_rn(double a, double b) { return a * b; }
+inline double __dadd_rn(double a, double b) { return a + b; }
+inline double __dsub_rn(double a, double b) { return a - b; }
 inline float exp2f_emu(float x) { return std::exp2(x); }
 inline int __float_as_int(float f) { int i; std::memcpy(&i, &f, 4); return i; }
 inline float __int_as_float(int i) { float f; std::memcpy(&f, &i, 4); return f; }
