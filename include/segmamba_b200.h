@@ -516,6 +516,59 @@ typedef struct smb_metric_select_args {
 
 SMB_API int smb_metric_select(const smb_metric_select_args *args, void *cuda_stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Case prediction on the GPU (segmamba_b200/predict.py): the steps of the reference's Predictor after the sliding window,
+ * plus exact 6-connected component post-processing.  All calls enqueue on `cuda_stream`, allocate nothing, never synchronise
+ * with the host, size their launches from shapes only and give bitwise-deterministic results.
+ *   smb_pred_restore  logits -> trilinear resample to the crop shape (F.interpolate, align_corners=False, fp32, stored as
+ *                     fp16) -> argmax -> label map or region masks, uncropped into the original volume, in one pass
+ *   smb_pred_cc       6-connected labelling of `batch` independent uint8 volumes (nonzero = foreground) and the three
+ *                     operations built on it (SMB_PRED_LABEL / _FILL_HOLES / _LARGEST)
+ * Volumes are limited to d * h * w < 2^31 voxels.
+ * ---------------------------------------------------------------------------------------------- */
+
+/* out[v] for v in (D0, H0, W0): 0 outside the box [z0, z0 + cd) x [y0, y0 + ch) x [x0, x0 + cw); inside, the argmax over
+ * c < classes (first maximum; a NaN is the maximum) of fp16(trilinear sample of channel c at the box coordinate, sampling the
+ * (d, h, w) logits as an output of size (cd, ch, cw)).  An axis whose crop size equals the logit size is copied.  Channel c
+ * of logit voxel u is src[c * class_stride + u * voxel_stride] (elements; dtype SMB_F32 / SMB_F16 / SMB_BF16).
+ * regions == 0: out is a (D0, H0, W0) uint8 label map; regions R in 1..8: out is (R, D0, H0, W0) uint8 with
+ * out[r, v] = bit r of lut[label] (0 for labels >= 256). */
+typedef struct smb_pred_restore_args {
+    const void *src;
+    void *out;
+    int64_t class_stride, voxel_stride;
+    int32_t dtype, classes, regions;
+    int32_t d, h, w;            /* logit volume */
+    int32_t cd, ch, cw;         /* crop shape (shape_after_cropping_before_resample) */
+    int32_t z0, y0, x0;         /* lower corner of bbox_used_for_cropping */
+    int32_t D0, H0, W0;         /* shape_before_cropping */
+    uint8_t lut[256];
+} smb_pred_restore_args;
+
+SMB_API int smb_pred_restore(const smb_pred_restore_args *args, void *cuda_stream);
+
+/* Components are 6-connected (scipy.ndimage.generate_binary_structure(3, 1)).
+ *   SMB_PRED_LABEL       out: (batch, d, h, w) int32 labels, 0 background, component k numbered by the raster order of its
+ *                        first voxel (scipy.ndimage.label's numbering); counts[b]: number of components (int64)
+ *   SMB_PRED_FILL_HOLES  out: (batch, d, h, w) uint8, scipy.ndimage.binary_fill_holes: the mask plus every background
+ *                        component without a voxel on the volume boundary
+ *   SMB_PRED_LARGEST     out: (batch, d, h, w) uint8, the holes-filled largest component (ties: the highest label); all zero
+ *                        for an empty mask.  counts is not used by the last two, and their out may be the mask itself.
+ * workspace: at least smb_pred_cc_workspace_bytes(batch, d, h, w) bytes, 16-byte aligned. */
+enum { SMB_PRED_LABEL = 0, SMB_PRED_FILL_HOLES = 1, SMB_PRED_LARGEST = 2 };
+
+typedef struct smb_pred_cc_args {
+    const void *mask;           /* (batch, d, h, w) uint8 */
+    void *out;
+    int64_t *counts;            /* (batch,), SMB_PRED_LABEL only */
+    void *workspace;
+    size_t workspace_bytes;
+    int32_t batch, d, h, w, op;
+} smb_pred_cc_args;
+
+SMB_API size_t smb_pred_cc_workspace_bytes(int32_t batch, int32_t d, int32_t h, int32_t w);
+SMB_API int smb_pred_cc(const smb_pred_cc_args *args, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

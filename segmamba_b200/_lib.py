@@ -180,6 +180,21 @@ METRIC_MAX_REGIONS, METRIC_MAX_AXIS, METRIC_NCOUNTS = 8, 768, 8
 METRIC_I8, METRIC_U8, METRIC_I32, METRIC_I64, METRIC_LOGITS = 0, 1, 2, 3, 4
 
 
+# case prediction (include/segmamba_b200.h, "Case prediction on the GPU")
+class PredRestoreArgs(ctypes.Structure):
+    _fields_ = ([("src", _vp), ("out", _vp), ("class_stride", _i64), ("voxel_stride", _i64)]
+                + [(n, _i32) for n in ("dtype", "classes", "regions", "d", "h", "w", "cd", "ch", "cw", "z0", "y0", "x0",
+                                       "D0", "H0", "W0")] + [("lut", ctypes.c_uint8 * 256)])
+
+
+class PredCcArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("mask", "out", "counts", "workspace")] + [("workspace_bytes", _sz)]
+                + [(n, _i32) for n in ("batch", "d", "h", "w", "op")])
+
+
+PRED_LABEL, PRED_FILL_HOLES, PRED_LARGEST = 0, 1, 2
+
+
 # every symbol include/segmamba_b200.h declares (tests/test_abi.py checks the header against this list)
 EXPORTS = {
     "smb_version": (ctypes.c_int, []),
@@ -211,6 +226,9 @@ EXPORTS = {
     "smb_metric_count": (ctypes.c_int, [ctypes.POINTER(MetricCountArgs), _vp]),
     "smb_metric_edt": (ctypes.c_int, [ctypes.POINTER(MetricEdtArgs), _vp]),
     "smb_metric_select": (ctypes.c_int, [ctypes.POINTER(MetricSelectArgs), _vp]),
+    "smb_pred_restore": (ctypes.c_int, [ctypes.POINTER(PredRestoreArgs), _vp]),
+    "smb_pred_cc_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
+    "smb_pred_cc": (ctypes.c_int, [ctypes.POINTER(PredCcArgs), _vp]),
 }
 
 _lib = None

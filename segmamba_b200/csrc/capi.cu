@@ -12,6 +12,7 @@
 #include "gemm_internal.h"
 #include "metrics_internal.h"
 #include "norm_internal.h"
+#include "predict_internal.h"
 #include "scan_internal.h"
 
 namespace smb {
@@ -593,6 +594,45 @@ SMB_API int smb_metric_select(const smb_metric_select_args *a, void *cuda_stream
     if (!(a->frac >= 0.0 && a->frac <= 1.0)) return fail(SMB_EINVAL, "smb_metric_select: frac must be in [0, 1]");
     cudaError_t e = smb::metric_select_launch(*a, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_metric_select");
+    return SMB_OK;
+}
+
+// case prediction (predict.cu)
+SMB_API int smb_pred_restore(const smb_pred_restore_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_pred_restore: null args");
+    if (!a->src || !a->out) return fail(SMB_EINVAL, "smb_pred_restore: src and out are required");
+    if (a->dtype < SMB_F32 || a->dtype > SMB_BF16) return fail(SMB_EINVAL, "smb_pred_restore: bad dtype %d", a->dtype);
+    if (a->classes <= 0 || a->classes > 256) return fail(SMB_EINVAL, "smb_pred_restore: classes must be 1..256");
+    if (a->class_stride <= 0 || a->voxel_stride <= 0) return fail(SMB_EINVAL, "smb_pred_restore: strides must be positive");
+    if (a->regions < 0 || a->regions > SMB_METRIC_MAX_REGIONS) return fail(SMB_EINVAL, "smb_pred_restore: regions must be 0..%d", SMB_METRIC_MAX_REGIONS);
+    if (a->d <= 0 || a->h <= 0 || a->w <= 0 || a->cd <= 0 || a->ch <= 0 || a->cw <= 0 || a->D0 <= 0 || a->H0 <= 0 || a->W0 <= 0)
+        return fail(SMB_EINVAL, "smb_pred_restore: every axis must be positive");
+    if (a->z0 < 0 || a->y0 < 0 || a->x0 < 0 || (int64_t)a->z0 + a->cd > a->D0 || (int64_t)a->y0 + a->ch > a->H0 || (int64_t)a->x0 + a->cw > a->W0)
+        return fail(SMB_EINVAL, "smb_pred_restore: the crop box must lie inside the original volume");
+    if ((int64_t)a->d * a->h * a->w > INT32_MAX || (int64_t)a->D0 * a->H0 * a->W0 > INT32_MAX)
+        return fail(SMB_EUNSUPPORTED, "smb_pred_restore: volumes are limited to 2^31 - 1 voxels");
+    cudaError_t e = smb::pred_restore_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_pred_restore");
+    return SMB_OK;
+}
+
+SMB_API size_t smb_pred_cc_workspace_bytes(int32_t batch, int32_t d, int32_t h, int32_t w) {
+    if (batch <= 0 || d <= 0 || h <= 0 || w <= 0) return 0;
+    return smb::pred_cc_workspace_bytes(batch, d, h, w);
+}
+
+SMB_API int smb_pred_cc(const smb_pred_cc_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_pred_cc: null args");
+    if (!a->mask || !a->out) return fail(SMB_EINVAL, "smb_pred_cc: mask and out are required");
+    if (a->batch <= 0 || a->batch > 65535 || a->d <= 0 || a->h <= 0 || a->w <= 0)
+        return fail(SMB_EINVAL, "smb_pred_cc: batch (1..65535) and axes must be positive");
+    if ((int64_t)a->d * a->h * a->w > INT32_MAX) return fail(SMB_EUNSUPPORTED, "smb_pred_cc: volumes are limited to 2^31 - 1 voxels");
+    if (a->op < SMB_PRED_LABEL || a->op > SMB_PRED_LARGEST) return fail(SMB_EINVAL, "smb_pred_cc: bad op %d", a->op);
+    if (a->op == SMB_PRED_LABEL && !a->counts) return fail(SMB_EINVAL, "smb_pred_cc: labelling needs counts");
+    if (!a->workspace || ((uintptr_t)a->workspace & 15) || a->workspace_bytes < smb::pred_cc_workspace_bytes(a->batch, a->d, a->h, a->w))
+        return fail(SMB_EWORKSPACE, "smb_pred_cc: workspace missing, misaligned or smaller than smb_pred_cc_workspace_bytes");
+    cudaError_t e = smb::pred_cc_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_pred_cc");
     return SMB_OK;
 }
 

@@ -208,6 +208,26 @@ inline unsigned atomicAdd(unsigned *addr, unsigned val) { return __atomic_fetch_
 inline unsigned long long atomicAdd(unsigned long long *addr, unsigned long long val) {
     return __atomic_fetch_add(addr, val, __ATOMIC_RELAXED);
 }
+inline int atomicMin(int *addr, int val) {
+    int old = __atomic_load_n(addr, __ATOMIC_RELAXED);
+    while (val < old && !__atomic_compare_exchange_n(addr, &old, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+    return old;
+}
+inline unsigned long long atomicMax(unsigned long long *addr, unsigned long long val) {
+    unsigned long long old = __atomic_load_n(addr, __ATOMIC_RELAXED);
+    while (val > old && !__atomic_compare_exchange_n(addr, &old, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+    return old;
+}
+inline int __popc(unsigned x) { return __builtin_popcount(x); }
+inline int __ffs(int x) { return __builtin_ffs(x); }
+// the lanes named by mask whose value equals this lane's
+template <typename T> inline unsigned __match_any_sync(unsigned mask, T v) {
+    uint64_t *slots = emu::warp_exchange(mask, emu::pack(v));
+    unsigned r = 0;
+    for (int l = 0; l < 32; ++l)
+        if (((mask >> l) & 1) && emu::lane_live_and_in_mask(l, mask) && slots[l] == emu::pack(v)) r |= 1u << l;
+    return r;
+}
 inline void __threadfence() { std::atomic_thread_fence(std::memory_order_seq_cst); }
 inline void __threadfence_block() { std::atomic_thread_fence(std::memory_order_seq_cst); }
 
