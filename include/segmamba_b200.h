@@ -20,6 +20,8 @@
  *   smb_gemm          the pointwise contractions (library GEMMs / 1x1x1 cuDNN convolutions in the reference):
  *                     Mamba.in_proj / out_proj  mamba_simple.py:204-208,264;  MlpChannel.fc1 / fc2  segmamba.py:81-89;
  *                     GSC.proj3 / proj4  segmamba.py:103-107;  UnetResBlock.conv3  dynunet_block.py:66-69
+ *   smb_conv3d*       the dense 3x3x3 convolutions (cuDNN in the reference): UnetResBlock.conv1 / conv2
+ *                     (dynunet_block.py) and GSC.proj / proj2 (segmamba.py)
  *
  * Scope (SURVEY.md section 8): real A, input-dependent ("variable") B and C, dstate in {8, 16},
  * conv width 2..4, non-channel-last conv layout, fp32 / fp16 / bf16 I/O with fp32 arithmetic.
@@ -303,6 +305,31 @@ typedef struct smb_gemm_args {
 } smb_gemm_args;
 
 SMB_API int smb_gemm(const smb_gemm_args *args, void *cuda_stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * 3x3x3 convolution, stride 1, padding 1, no bias, on channels-last activations (implicit GEMM on wgmma; no im2col):
+ *   smb_conv3d        y[n, d, h, w, co] = sum_{kd,kh,kw,ci} x[n, d+kd-1, h+kh-1, w+kw-1, ci] . weight[co, kd, kh, kw, ci]
+ *                     (zero outside the volume).  The data gradient is this call on dy with the weight flipped in kd, kh, kw
+ *                     and its two channel axes swapped (c_in and c_out swapped as well).
+ *   smb_conv3d_wgrad  dweight[co, kd, kh, kw, ci] += sum_{n,d,h,w} dy[n, d, h, w, co] . x[n, d+kd-1, h+kh-1, w+kw-1, ci]
+ *                     dweight is fp32 and accumulated into (zero it first); the summation order varies between runs.
+ * x (batch, d, h, w, c_in), y / dy (batch, d, h, w, c_out): contiguous, fp16 or bf16 (dtype), 16-byte aligned; weight
+ * (c_out, 3, 3, 3, c_in) contiguous in the same dtype.  c_in and c_out: multiples of 8.  The number of kernel launches
+ * depends only on the shapes, nothing synchronises with the host.
+ * ------------------------------------------------------------------------------------------------ */
+typedef struct smb_conv3d_args {
+    int32_t batch, d, h, w;
+    int32_t c_in, c_out;
+    int32_t dtype;              /* SMB_F16 / SMB_BF16 */
+    const void *x;
+    const void *weight;         /* smb_conv3d */
+    void *y;                    /* smb_conv3d */
+    const void *dy;             /* smb_conv3d_wgrad */
+    float *dweight;             /* smb_conv3d_wgrad */
+} smb_conv3d_args;
+
+SMB_API int smb_conv3d(const smb_conv3d_args *args, void *cuda_stream);
+SMB_API int smb_conv3d_wgrad(const smb_conv3d_args *args, void *cuda_stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Strided 2-D copy, 16-byte vectors: `rows` rows of `row_bytes` bytes from src (row pitch src_pitch_bytes) to dst (row

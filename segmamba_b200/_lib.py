@@ -102,6 +102,11 @@ class GemmArgs(ctypes.Structure):
                 + [(n, _vp) for n in ("A", "B", "bias", "D")] + [(n, _i64) for n in ("lda", "ldb", "ldd")])
 
 
+class Conv3dArgs(ctypes.Structure):
+    _fields_ = ([(n, _i32) for n in ("batch", "d", "h", "w", "c_in", "c_out", "dtype")]
+                + [(n, _vp) for n in ("x", "weight", "y", "dy", "dweight")])
+
+
 # training-patch augmentation (include/segmamba_b200.h, "Training-patch sampling and augmentation")
 _f64, _f32 = ctypes.c_double, ctypes.c_float
 
@@ -214,6 +219,8 @@ EXPORTS = {
     "smb_layernorm_fwd": (ctypes.c_int, [ctypes.POINTER(LayerNormArgs), _vp]),
     "smb_layernorm_bwd": (ctypes.c_int, [ctypes.POINTER(LayerNormBwdArgs), _vp]),
     "smb_gemm": (ctypes.c_int, [ctypes.POINTER(GemmArgs), _vp]),
+    "smb_conv3d": (ctypes.c_int, [ctypes.POINTER(Conv3dArgs), _vp]),
+    "smb_conv3d_wgrad": (ctypes.c_int, [ctypes.POINTER(Conv3dArgs), _vp]),
     "smb_copy2d": (ctypes.c_int, [_vp, _i64, _vp, _i64, _i64, _i64, _vp]),
     "smb_aug_crop": (ctypes.c_int, [ctypes.POINTER(AugCropArgs), _vp]),
     "smb_aug_prefilter": (ctypes.c_int, [ctypes.POINTER(AugPrefilterJob), _i32, _vp]),

@@ -8,6 +8,7 @@
 
 #include "../../include/segmamba_b200.h"
 #include "aug_internal.h"
+#include "conv3d_internal.h"
 #include "conv_internal.h"
 #include "gemm_internal.h"
 #include "metrics_internal.h"
@@ -22,6 +23,7 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 // wgmma / TMA have no CPU emulation: the emulated library exports smb_gemm but every call fails loudly
 cudaError_t gemm_tc_launch(GemmP, const void *, int64_t, const void *, int64_t, cudaStream_t, const char **) { return cudaErrorNotSupported; }
 int gemm_pick_bn(int) { return 0; }
+cudaError_t conv3d_tc_launch(Conv3dP, const void *, const void *, cudaStream_t, const char **) { return cudaErrorNotSupported; }
 #endif
 }  // namespace smb
 
@@ -418,6 +420,44 @@ SMB_API int smb_gemm(const smb_gemm_args *a, void *cuda_stream) {
         return fail(SMB_ECUDA, "smb_gemm: %s failed: CUDA error %d (%s) [M=%d N=%d K=%d a_major=%d b_major=%d lda=%lld ldb=%lld]", where,
                     (int)e, cudaGetErrorString(e), a->M, a->N, a->K, a->a_major, a->b_major, (long long)a->lda, (long long)a->ldb);
     return SMB_OK;
+}
+
+namespace {
+int conv3d_check(const char *fn, const smb_conv3d_args *a, const void *x, const void *b, const void *out) {
+    if (!a) return fail(SMB_EINVAL, "%s: null args", fn);
+    if (!x || !b || !out) return fail(SMB_EINVAL, "%s: all tensors are required", fn);
+    if (a->batch <= 0 || a->d <= 0 || a->h <= 0 || a->w <= 0) return fail(SMB_EINVAL, "%s: extents must be positive", fn);
+    if (a->dtype != SMB_F16 && a->dtype != SMB_BF16) return fail(SMB_EUNSUPPORTED, "%s: operands must be fp16 or bf16", fn);
+    if (a->c_in <= 0 || a->c_out <= 0 || (a->c_in % 8) || (a->c_out % 8))
+        return fail(SMB_EUNSUPPORTED, "%s: c_in and c_out must be positive multiples of 8 (16-byte rows for TMA)", fn);
+    if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(b) & 15))
+        return fail(SMB_EINVAL, "%s: operands must be 16-byte aligned", fn);
+    if ((int64_t)a->batch * a->d * a->h * a->w >= (int64_t)1 << 31) return fail(SMB_EINVAL, "%s: more than 2^31 voxels", fn);
+    return SMB_OK;
+}
+
+int conv3d_run(const char *fn, const smb_conv3d_args *a, int wgrad, const void *x, const void *b, void *out, void *cuda_stream) {
+    smb::Conv3dP p;
+    memset(&p, 0, sizeof(p));
+    p.batch = a->batch; p.D = a->d; p.H = a->h; p.W = a->w; p.C_in = a->c_in; p.C_out = a->c_out;
+    p.dtype = a->dtype; p.wgrad = wgrad; p.out = out;
+    const char *where = "";
+    cudaError_t e = smb::conv3d_tc_launch(p, x, b, (cudaStream_t)cuda_stream, &where);
+    if (e != cudaSuccess)
+        return fail(SMB_ECUDA, "%s: %s failed: CUDA error %d (%s) [batch=%d d=%d h=%d w=%d c_in=%d c_out=%d]", fn, where, (int)e,
+                    cudaGetErrorString(e), a->batch, a->d, a->h, a->w, a->c_in, a->c_out);
+    return SMB_OK;
+}
+}  // namespace
+
+SMB_API int smb_conv3d(const smb_conv3d_args *a, void *cuda_stream) {
+    int rc = conv3d_check("smb_conv3d", a, a ? a->x : nullptr, a ? a->weight : nullptr, a ? a->y : nullptr);
+    return rc != SMB_OK ? rc : conv3d_run("smb_conv3d", a, 0, a->x, a->weight, a->y, cuda_stream);
+}
+
+SMB_API int smb_conv3d_wgrad(const smb_conv3d_args *a, void *cuda_stream) {
+    int rc = conv3d_check("smb_conv3d_wgrad", a, a ? a->x : nullptr, a ? a->dy : nullptr, a ? a->dweight : nullptr);
+    return rc != SMB_OK ? rc : conv3d_run("smb_conv3d_wgrad", a, 1, a->x, a->dy, a->dweight, cuda_stream);
 }
 
 SMB_API int smb_copy2d(const void *src, int64_t src_pitch_bytes, void *dst, int64_t dst_pitch_bytes, int64_t rows, int64_t row_bytes,

@@ -7,8 +7,10 @@ Module / attribute names reproduce the reference's 291 state_dict keys (SURVEY.m
 ``decoder{5..2}.{transp_conv.conv,conv_block.conv{1,2,3}.conv}``, ``decoder1.layer.conv{1,2}.conv``, ``out.conv.conv``.
 The MONAI blocks are restated minimally (monai/networks/blocks/dynunet_block.py:25-111,247-267,
 unetr_block.py:22-86,209-259, convolutions.py:25): dense Conv3d / ConvTranspose3d(k2,s2) without bias,
-InstanceNorm3d(affine=False, eps=1e-5), LeakyReLU(0.01).  The dense 3-D convolutions are library (cuDNN) calls,
-as in the reference; the TSMamba token mixer and every InstanceNorm(+activation+residual) chain are native kernels.
+InstanceNorm3d(affine=False, eps=1e-5), LeakyReLU(0.01).  The dense 3x3x3 convolutions of UnetResBlock and GSC run on the
+native implicit-GEMM kernel where conv3d.native_ok allows it (16-bit compute, large volumes); the other dense convolutions
+are library (cuDNN) calls, as in the reference.  The TSMamba token mixer and every InstanceNorm(+activation+residual) chain
+are native kernels.
 
 Data layout: activations are kept channels-last (NDHWC) end to end, so (i) cuDNN's tensor-core convolutions need
 no NCHW<->NHWC conversion kernels, (ii) the (B, L, C) token view that MambaLayer needs is free (the reference pays a
@@ -21,6 +23,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import gemm as _gemm
+from . import conv3d as _conv3d
 from . import layer_norm
 from . import layout as _layout
 from .instance_norm import fused_instance_norm
@@ -64,11 +67,11 @@ def _conv_before_norm(conv: nn.Conv3d, x: torch.Tensor) -> torch.Tensor:
     convolution) nor reduced in the backward (one reduction per convolution); the parameter stays in the graph with an exact
     zero gradient, so weight decay acts on it exactly as in the reference and the state_dict surface is unchanged."""
     if conv.bias is None:
-        return _pointwise(conv, x) if conv.kernel_size == (1, 1, 1) else conv(x)
+        return _pointwise(conv, x) if conv.kernel_size == (1, 1, 1) else _conv3d.conv3d(conv, x)
     if conv.kernel_size == (1, 1, 1) and _gemm.MODE == "all":
         y = _pointwise(_BiasFree(conv), x)
     else:
-        y = F.conv3d(x, conv.weight, None, conv.stride, conv.padding, conv.dilation, conv.groups)
+        y = _conv3d.conv3d(conv, x, bias=False)
     return _ZeroGradBias.apply(y, conv.bias)
 
 
@@ -115,8 +118,8 @@ class UnetResBlock(nn.Module):
 
     def forward(self, inp):
         # norm1/norm2/norm3/lrelu stay registered for structural parity; the math runs in the fused kernels
-        out = fused_instance_norm(self.conv1.conv(inp), "leaky_relu", 0.01)   # dynunet_block.py:100-102
-        out = self.conv2(out)
+        out = fused_instance_norm(_conv3d.conv3d(self.conv1.conv, inp), "leaky_relu", 0.01)   # dynunet_block.py:100-102
+        out = _conv3d.conv3d(self.conv2.conv, out)
         if self.downsample:                                                               # :105-110
             return fused_instance_norm(out, "leaky_relu", 0.01, add=_pointwise(self.conv3.conv, inp), add_norm=True)
         return fused_instance_norm(out, "leaky_relu", 0.01, add=inp)
