@@ -596,6 +596,109 @@ typedef struct smb_pred_cc_args {
 SMB_API size_t smb_pred_cc_workspace_bytes(int32_t batch, int32_t d, int32_t h, int32_t w);
 SMB_API int smb_pred_cc(const smb_pred_cc_args *args, void *cuda_stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Case preprocessing on the GPU (segmamba_b200/preprocess.py): the reference's DefaultPreprocessor.run_case_npy (nonzero
+ * crop with hole filling, z-score, resampling to the target spacing, foreground locations) and
+ * collect_foreground_intensities.  The hole filling is smb_pred_cc (SMB_PRED_FILL_HOLES) and the cubic data resize is
+ * smb_aug_stats + smb_aug_prefilter (SMB_AUG_EDGE) + smb_aug_resample (SMB_AUG_ZOOM, clipped); the calls here are the rest.
+ * All enqueue on `cuda_stream`, allocate nothing, never synchronise with the host, size their launches from shapes only
+ * and give bitwise-deterministic results.  Volumes are limited to d * h * w < 2^31 voxels.
+ * ---------------------------------------------------------------------------------------------- */
+#define SMB_PREP_CHUNK 1024           /* voxels per chunk of the ordered compaction */
+#define SMB_PREP_MAX_JOBS 8           /* jobs per smb_prep_count / smb_prep_compact / smb_prep_normalize launch */
+
+/* reductions of smb_prep_mask (the call zeroes the record first) */
+typedef struct smb_prep_record {
+    int64_t lo_flip0, lo_flip1, lo_flip2;   /* 2^31 - (lowest index of a nonzero voxel) per axis; 0 when none */
+    int64_t hi0, hi1, hi2;                  /* highest index of a nonzero voxel + 1 per axis; 0 when none */
+    int64_t foreground;                     /* voxels with seg > 0 */
+    int64_t nan_voxels;                     /* voxels with a NaN in some channel */
+    int64_t bad_labels;                     /* seg voxels that are not an integer in [0, 127] (NaN included) */
+} smb_prep_record;
+
+/* mask[v] = 1 where some channel of data is nonzero (a NaN is nonzero), seg8[v] = int8 of seg[v] (0 without seg), plus the
+ * record.  data (channels, d, h, w) fp32, seg (d, h, w) fp32 or NULL. */
+typedef struct smb_prep_mask_args {
+    const float *data;
+    const float *seg;
+    uint8_t *mask;
+    int8_t *seg8;
+    smb_prep_record *record;
+    int32_t channels, d, h, w;
+} smb_prep_mask_args;
+
+SMB_API int smb_prep_mask(const smb_prep_mask_args *args, void *cuda_stream);
+
+/* The box [z0, z0 + cd) x [y0, y0 + ch) x [x0, x0 + cw) of the (d, h, w) volume: out (channels, cd, ch, cw) fp32 copies data,
+ * seg_out (cd, ch, cw) int8 is seg8 with nonzero_label where seg8 is 0 and mask is 0 (crop_to_nonzero's relabel). */
+typedef struct smb_prep_crop_args {
+    const float *data;
+    const uint8_t *mask;
+    const int8_t *seg8;
+    float *out;
+    int8_t *seg_out;
+    int32_t channels, d, h, w, z0, y0, x0, cd, ch, cw;
+    int32_t nonzero_label;      /* -128..127 */
+} smb_prep_crop_args;
+
+SMB_API int smb_prep_crop(const smb_prep_crop_args *args, void *cuda_stream);
+
+/* ZScoreNormalization(use_mask_for_norm=False) of one channel of n voxels from its smb_aug_stats record:
+ * dst = fp32((src - mean) / max(std, 1e-8)) in fp64, mean = sum / n, std = sqrt(max(sumsq / n - mean^2, 0));
+ * moments[0..1] = mean, std.  dst may be src. */
+typedef struct smb_prep_norm_job {
+    const float *src;
+    float *dst;
+    const double *stats;
+    double *moments;
+    int64_t n;
+} smb_prep_norm_job;
+
+SMB_API int smb_prep_normalize(const smb_prep_norm_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* batchgenerators resize_segmentation(order=1) of an int8 label volume (n0, n1, n2) -> (m0, m1, m2): per output voxel and per
+ * axis the coordinate (o + 0.5) n / m - 0.5 clamped to [0, n - 1] (scipy zoom, grid_mode, mode 'nearest'), the trilinear
+ * indicator of every label among the 8 taps in fp64, and the highest label whose indicator is >= 0.5 wins (0 when none). */
+typedef struct smb_prep_label_resize_args {
+    const int8_t *src;
+    int8_t *dst;
+    int32_t n0, n1, n2, m0, m1, m2;
+} smb_prep_label_resize_args;
+
+SMB_API int smb_prep_label_resize(const smb_prep_label_resize_args *args, void *cuda_stream);
+
+/* Ordered compaction of the voxels of an int8 volume whose label is in a set (bit (uint8_t)label of `set`).
+ *   smb_prep_count    chunk[k] = matching voxels of chunk k before it (exclusive scan), *count = total
+ *   smb_prep_compact  index[0 .. count) = linear indices of the matching voxels in raster order, from the chunk offsets of
+ *                     smb_prep_count on the same job (index holds at least count entries) */
+typedef struct smb_prep_compact_job {
+    const int8_t *seg;
+    int32_t *chunk;             /* ceil(n / SMB_PREP_CHUNK) ints */
+    int64_t *count;
+    int32_t *index;             /* smb_prep_compact only */
+    int64_t n;
+    uint32_t set[8];
+} smb_prep_compact_job;
+
+SMB_API int smb_prep_count(const smb_prep_compact_job *jobs, int32_t n_jobs, void *cuda_stream);
+SMB_API int smb_prep_compact(const smb_prep_compact_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* i in [0, n), p = index[select ? select[i] : i] (select entries must lie in [0, index length)):
+ *   rows    (rows != NULL)    rows[4 i .. 4 i + 3] = 0, z, y, x of p in a (d, h, w) volume (np.argwhere of a (1, d, h, w) array)
+ *   values  (values != NULL)  values[c n + i] = data[c channel_stride + p] for c < channels; with select_channel_stride s,
+ *                             channel c reads select[c s + i] instead (s = 0: one selection for all channels) */
+typedef struct smb_prep_gather_args {
+    const int32_t *index;
+    const int64_t *select;
+    int64_t *rows;
+    const float *data;
+    float *values;
+    int64_t n, channel_stride, select_channel_stride;
+    int32_t channels, d, h, w;
+} smb_prep_gather_args;
+
+SMB_API int smb_prep_gather(const smb_prep_gather_args *args, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -200,6 +200,42 @@ class PredCcArgs(ctypes.Structure):
 PRED_LABEL, PRED_FILL_HOLES, PRED_LARGEST = 0, 1, 2
 
 
+# case preprocessing (include/segmamba_b200.h, "Case preprocessing on the GPU")
+class PrepRecord(ctypes.Structure):
+    _fields_ = [(n, _i64) for n in ("lo_flip0", "lo_flip1", "lo_flip2", "hi0", "hi1", "hi2", "foreground", "nan_voxels",
+                                    "bad_labels")]
+
+
+class PrepMaskArgs(ctypes.Structure):
+    _fields_ = [(n, _vp) for n in ("data", "seg", "mask", "seg8", "record")] + [(n, _i32) for n in ("channels", "d", "h", "w")]
+
+
+class PrepCropArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("data", "mask", "seg8", "out", "seg_out")]
+                + [(n, _i32) for n in ("channels", "d", "h", "w", "z0", "y0", "x0", "cd", "ch", "cw", "nonzero_label")])
+
+
+class PrepNormJob(ctypes.Structure):
+    _fields_ = [(n, _vp) for n in ("src", "dst", "stats", "moments")] + [("n", _i64)]
+
+
+class PrepLabelResizeArgs(ctypes.Structure):
+    _fields_ = [("src", _vp), ("dst", _vp)] + [(n, _i32) for n in ("n0", "n1", "n2", "m0", "m1", "m2")]
+
+
+class PrepCompactJob(ctypes.Structure):
+    _fields_ = [(n, _vp) for n in ("seg", "chunk", "count", "index")] + [("n", _i64), ("set", ctypes.c_uint32 * 8)]
+
+
+class PrepGatherArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("index", "select", "rows", "data", "values")]
+                + [(n, _i64) for n in ("n", "channel_stride", "select_channel_stride")]
+                + [(n, _i32) for n in ("channels", "d", "h", "w")])
+
+
+PREP_CHUNK, PREP_MAX_JOBS = 1024, 8
+
+
 # every symbol include/segmamba_b200.h declares (tests/test_abi.py checks the header against this list)
 EXPORTS = {
     "smb_version": (ctypes.c_int, []),
@@ -236,6 +272,13 @@ EXPORTS = {
     "smb_pred_restore": (ctypes.c_int, [ctypes.POINTER(PredRestoreArgs), _vp]),
     "smb_pred_cc_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
     "smb_pred_cc": (ctypes.c_int, [ctypes.POINTER(PredCcArgs), _vp]),
+    "smb_prep_mask": (ctypes.c_int, [ctypes.POINTER(PrepMaskArgs), _vp]),
+    "smb_prep_crop": (ctypes.c_int, [ctypes.POINTER(PrepCropArgs), _vp]),
+    "smb_prep_normalize": (ctypes.c_int, [ctypes.POINTER(PrepNormJob), _i32, _vp]),
+    "smb_prep_label_resize": (ctypes.c_int, [ctypes.POINTER(PrepLabelResizeArgs), _vp]),
+    "smb_prep_count": (ctypes.c_int, [ctypes.POINTER(PrepCompactJob), _i32, _vp]),
+    "smb_prep_compact": (ctypes.c_int, [ctypes.POINTER(PrepCompactJob), _i32, _vp]),
+    "smb_prep_gather": (ctypes.c_int, [ctypes.POINTER(PrepGatherArgs), _vp]),
 }
 
 _lib = None

@@ -14,6 +14,7 @@
 #include "metrics_internal.h"
 #include "norm_internal.h"
 #include "predict_internal.h"
+#include "prep_internal.h"
 #include "scan_internal.h"
 
 namespace smb {
@@ -673,6 +674,98 @@ SMB_API int smb_pred_cc(const smb_pred_cc_args *a, void *cuda_stream) {
         return fail(SMB_EWORKSPACE, "smb_pred_cc: workspace missing, misaligned or smaller than smb_pred_cc_workspace_bytes");
     cudaError_t e = smb::pred_cc_launch(*a, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_pred_cc");
+    return SMB_OK;
+}
+
+// case preprocessing (preprocess.cu)
+static int prep_volume(int64_t d, int64_t h, int64_t w, const char *who) {
+    if (d <= 0 || h <= 0 || w <= 0) return fail(SMB_EINVAL, "%s: axes must be positive", who);
+    if (d * h * w > INT32_MAX) return fail(SMB_EUNSUPPORTED, "%s: volumes are limited to 2^31 - 1 voxels", who);
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_mask(const smb_prep_mask_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_prep_mask: null args");
+    if (!a->data || !a->mask || !a->seg8 || !a->record) return fail(SMB_EINVAL, "smb_prep_mask: data, mask, seg8, record are required");
+    if (a->channels <= 0) return fail(SMB_EINVAL, "smb_prep_mask: channels must be positive");
+    int rc = prep_volume(a->d, a->h, a->w, "smb_prep_mask");
+    if (rc != SMB_OK) return rc;
+    cudaError_t e = smb::prep_mask_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_mask");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_crop(const smb_prep_crop_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_prep_crop: null args");
+    if (!a->data || !a->mask || !a->seg8 || !a->out || !a->seg_out) return fail(SMB_EINVAL, "smb_prep_crop: data, mask, seg8, out, seg_out are required");
+    if (a->channels <= 0) return fail(SMB_EINVAL, "smb_prep_crop: channels must be positive");
+    int rc = prep_volume(a->d, a->h, a->w, "smb_prep_crop");
+    if (rc != SMB_OK) return rc;
+    if (a->cd <= 0 || a->ch <= 0 || a->cw <= 0 || a->z0 < 0 || a->y0 < 0 || a->x0 < 0 || (int64_t)a->z0 + a->cd > a->d ||
+        (int64_t)a->y0 + a->ch > a->h || (int64_t)a->x0 + a->cw > a->w)
+        return fail(SMB_EINVAL, "smb_prep_crop: the box must be non-empty and lie inside the volume");
+    if (a->nonzero_label < -128 || a->nonzero_label > 127) return fail(SMB_EINVAL, "smb_prep_crop: nonzero_label must fit int8");
+    cudaError_t e = smb::prep_crop_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_crop");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_normalize(const smb_prep_norm_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_prep_normalize: bad job list");
+    for (int q = 0; q < n_jobs; ++q)
+        if (!jobs[q].src || !jobs[q].dst || !jobs[q].stats || !jobs[q].moments || jobs[q].n <= 0)
+            return fail(SMB_EINVAL, "smb_prep_normalize: job %d: src, dst, stats, moments, n > 0 required", q);
+    cudaError_t e = smb::prep_normalize_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_normalize");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_label_resize(const smb_prep_label_resize_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_prep_label_resize: null args");
+    if (!a->src || !a->dst) return fail(SMB_EINVAL, "smb_prep_label_resize: src and dst are required");
+    int rc = prep_volume(a->n0, a->n1, a->n2, "smb_prep_label_resize");
+    if (rc == SMB_OK) rc = prep_volume(a->m0, a->m1, a->m2, "smb_prep_label_resize");
+    if (rc != SMB_OK) return rc;
+    cudaError_t e = smb::prep_label_resize_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_label_resize");
+    return SMB_OK;
+}
+
+static int prep_jobs(const smb_prep_compact_job *jobs, int32_t n_jobs, bool compact, const char *who) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "%s: bad job list", who);
+    for (int q = 0; q < n_jobs; ++q) {
+        const smb_prep_compact_job &j = jobs[q];
+        if (!j.seg || !j.chunk || !j.count || (compact && !j.index)) return fail(SMB_EINVAL, "%s: job %d lacks a buffer", who, q);
+        if (j.n <= 0 || j.n > INT32_MAX) return fail(SMB_EUNSUPPORTED, "%s: job %d: n must be 1..2^31 - 1", who, q);
+    }
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_count(const smb_prep_compact_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    int rc = prep_jobs(jobs, n_jobs, false, "smb_prep_count");
+    if (rc != SMB_OK) return rc;
+    cudaError_t e = smb::prep_count_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_count");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_compact(const smb_prep_compact_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    int rc = prep_jobs(jobs, n_jobs, true, "smb_prep_compact");
+    if (rc != SMB_OK) return rc;
+    cudaError_t e = smb::prep_compact_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_compact");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_gather(const smb_prep_gather_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_prep_gather: null args");
+    if (!a->index || (!a->rows && !a->values)) return fail(SMB_EINVAL, "smb_prep_gather: index and rows or values are required");
+    if (a->n < 0) return fail(SMB_EINVAL, "smb_prep_gather: n must be non-negative");
+    if (a->rows && prep_volume(a->d, a->h, a->w, "smb_prep_gather") != SMB_OK) return SMB_EINVAL;
+    if (a->values && (!a->data || a->channels <= 0 || a->channel_stride < 0 || a->select_channel_stride < 0))
+        return fail(SMB_EINVAL, "smb_prep_gather: values need data, channels > 0 and non-negative strides");
+    cudaError_t e = smb::prep_gather_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_gather");
     return SMB_OK;
 }
 

@@ -23,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "segmamba_b200", "csrc")
 BUILD = os.path.join(HERE, "_build")
 OUT = os.path.join(BUILD, "libsegmamba_b200_emu.so")
-SOURCES = ["capi.cu", "scan_fwd.cu", "scan_fwd_v2.cu", "scan_bwd.cu", "scan_bwd_v2.cu", "scan_bwd_r3v2.cu", "conv1d.cu", "conv1d_v2.cu", "instnorm.cu", "layernorm.cu", "layout.cu", "augment.cu", "metrics.cu", "predict.cu"]
+SOURCES = ["capi.cu", "scan_fwd.cu", "scan_fwd_v2.cu", "scan_bwd.cu", "scan_bwd_v2.cu", "scan_bwd_r3v2.cu", "conv1d.cu", "conv1d_v2.cu", "instnorm.cu", "layernorm.cu", "layout.cu", "augment.cu", "metrics.cu", "predict.cu", "preprocess.cu"]
 CUDA_INC = os.environ.get("CUDA_HOME", "/usr/local/cuda") + "/include"
 
 
