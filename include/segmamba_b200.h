@@ -379,7 +379,8 @@ SMB_API int smb_aug_crop(const smb_aug_crop_args *args, void *cuda_stream);
 /* cubic B-spline coefficients of src (scipy.ndimage.spline_filter, order 3) on a grid with a 2-sample border per side:
  * coef is (n0 + 4, n1 + 4, n2 + 4).  SMB_AUG_MIRROR: whole-sample mirror boundary, the border holds the mirrored coefficients
  * (map_coordinates mode 'constant' / 'mirror');  SMB_AUG_EDGE: the coefficients of src padded by 12 edge samples per side and
- * filtered with the 'nearest' boundary, as scipy does for mode 'nearest' (zoom of skimage's resize, mode 'edge'). */
+ * filtered with the 'nearest' boundary, as scipy does for mode 'nearest' (zoom of skimage's resize, mode 'edge').
+ * Axes need at least 4 samples; SMB_AUG_MIRROR axes at most 256.  The grid is limited to 2^31 - 1 voxels. */
 typedef struct smb_aug_prefilter_job {
     const float *src;           /* (n0, n1, n2) */
     float *coef;                /* (n0 + 4, n1 + 4, n2 + 4); must not overlap src */
@@ -605,7 +606,7 @@ SMB_API int smb_pred_cc(const smb_pred_cc_args *args, void *cuda_stream);
  * and give bitwise-deterministic results.  Volumes are limited to d * h * w < 2^31 voxels.
  * ---------------------------------------------------------------------------------------------- */
 #define SMB_PREP_CHUNK 1024           /* voxels per chunk of the ordered compaction */
-#define SMB_PREP_MAX_JOBS 8           /* jobs per smb_prep_count / smb_prep_compact / smb_prep_normalize launch */
+#define SMB_PREP_MAX_JOBS 8           /* jobs per smb_prep_count / smb_prep_compact / smb_prep_normalize / smb_prep_ct_normalize launch */
 
 /* reductions of smb_prep_mask (the call zeroes the record first) */
 typedef struct smb_prep_record {
@@ -655,6 +656,19 @@ typedef struct smb_prep_norm_job {
 } smb_prep_norm_job;
 
 SMB_API int smb_prep_normalize(const smb_prep_norm_job *jobs, int32_t n_jobs, void *cuda_stream);
+
+/* CTNormalization(use_mask_for_norm=False) of one channel of n voxels from the dataset's foreground statistics, in fp32 as
+ * numpy computes it for a float32 image and Python-float properties: dst = (min(max(src, lo), hi) - mean) / div with IEEE
+ * rounding and no contraction (a NaN stays NaN), lo = fp32(percentile_00_5), hi = fp32(percentile_99_5), mean = fp32(mean),
+ * div = fp32(max(std, 1e-8)).  dst may be src.  At most SMB_PREP_MAX_JOBS jobs per launch; longer lists are split. */
+typedef struct smb_prep_ct_norm_job {
+    const float *src;
+    float *dst;
+    int64_t n;
+    float lo, hi, mean, div;
+} smb_prep_ct_norm_job;
+
+SMB_API int smb_prep_ct_normalize(const smb_prep_ct_norm_job *jobs, int32_t n_jobs, void *cuda_stream);
 
 /* batchgenerators resize_segmentation(order=1) of an int8 label volume (n0, n1, n2) -> (m0, m1, m2): per output voxel and per
  * axis the coordinate (o + 0.5) n / m - 0.5 clamped to [0, n - 1] (scipy zoom, grid_mode, mode 'nearest'), the trilinear

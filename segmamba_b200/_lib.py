@@ -219,6 +219,10 @@ class PrepNormJob(ctypes.Structure):
     _fields_ = [(n, _vp) for n in ("src", "dst", "stats", "moments")] + [("n", _i64)]
 
 
+class PrepCtNormJob(ctypes.Structure):
+    _fields_ = [("src", _vp), ("dst", _vp), ("n", _i64)] + [(n, ctypes.c_float) for n in ("lo", "hi", "mean", "div")]
+
+
 class PrepLabelResizeArgs(ctypes.Structure):
     _fields_ = [("src", _vp), ("dst", _vp)] + [(n, _i32) for n in ("n0", "n1", "n2", "m0", "m1", "m2")]
 
@@ -275,6 +279,7 @@ EXPORTS = {
     "smb_prep_mask": (ctypes.c_int, [ctypes.POINTER(PrepMaskArgs), _vp]),
     "smb_prep_crop": (ctypes.c_int, [ctypes.POINTER(PrepCropArgs), _vp]),
     "smb_prep_normalize": (ctypes.c_int, [ctypes.POINTER(PrepNormJob), _i32, _vp]),
+    "smb_prep_ct_normalize": (ctypes.c_int, [ctypes.POINTER(PrepCtNormJob), _i32, _vp]),
     "smb_prep_label_resize": (ctypes.c_int, [ctypes.POINTER(PrepLabelResizeArgs), _vp]),
     "smb_prep_count": (ctypes.c_int, [ctypes.POINTER(PrepCompactJob), _i32, _vp]),
     "smb_prep_compact": (ctypes.c_int, [ctypes.POINTER(PrepCompactJob), _i32, _vp]),

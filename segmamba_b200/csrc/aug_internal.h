@@ -11,8 +11,10 @@ namespace smb {
 // jobs per launch: the records travel by value in the kernel parameters (no host-to-device copy, no allocation, and the
 // caller's host array may be reused as soon as the entry point returns); longer lists are split into several launches
 constexpr int kAugMaxJobs = 8;
-// longest axis a prefilter line may have (the edge variant stages n + 24 samples per line in shared memory)
+// longest axis of a training patch (crop, blur, emit) and of a mirror-boundary prefilter line
 constexpr int kAugMaxAxis = 256;
+// longest prefilter line staged whole in shared memory (n + 24 samples per line); longer edge-boundary lines stream
+constexpr int kAugShortLine = 256;
 // blocks per stats job (partial sums land in the job's scratch, then one ordered reduction: deterministic)
 constexpr int kAugStatsBlocks = SMB_AUG_STATS_SCRATCH / 4;
 

@@ -4,7 +4,7 @@
 //
 // What bounds them: all are HBM-streaming passes over 4-byte voxels except the cubic resample (64 gathered taps per voxel out of
 // L1 / L2, the coefficient volume of one channel is 9 MB and stays resident in the 50 MB L2) and the prefilter (a two-pass
-// recursive filter per line, one thread per line, lines staged in shared memory).
+// recursive filter per line, one thread per line, lines of up to 256 samples staged in shared memory, longer ones streamed).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -108,6 +108,7 @@ __global__ void __launch_bounds__(32) prefilter_kernel(Jobs<smb_aug_prefilter_jo
     const int E1 = jb.n1 + 4, E2 = jb.n2 + 4;
     const int64_t es[3] = {(int64_t)E1 * E2, E2, 1};
     const int na = n[axis];
+    if (na > kAugShortLine) return;                                  // prefilter_long_*_kernel's line
     // lines of this axis: over the border-extended range of the axes already filtered, the valid range of the others
     const int r0 = axis == 0 ? jb.n1 : jb.n0 + 4;                    // outer line index range
     const int r1 = axis == 2 ? E1 : jb.n2;                           // inner line index range (axis 0: n2, axis 1: n2, axis 2: E1)
@@ -163,6 +164,169 @@ __global__ void __launch_bounds__(32) prefilter_kernel(Jobs<smb_aug_prefilter_jo
             const int q = edge ? p + pad : mirror_index(p, na);
             jb.coef[base + (int64_t)(p + 2) * es[axis]] = sm[q * 33 + t];
         }
+    }
+}
+
+// ---- cubic B-spline prefilter of lines longer than kAugShortLine, edge boundary -------------------------------------------------
+// filter_line's steps on the padded line q = p + 12 in [0, n + 24) without staging it: the 12 pad samples per side are the first
+// and last sample, so they are never stored.  The causal pass streams p = -2 .. n + 1 forward, writing c+ over the coefficient
+// grid, and keeps the 10 pad values past it in registers; the anticausal pass streams the grid range backward.  The recursion
+// state lives in a register, so shared memory does not grow with n.  The causal initial value is filter_line's 'nearest' sum:
+// for n + 24 > 280 samples z^(n+24) is 0 in fp32, so the terms of the far end vanish and the sum stops once z^q underflows.
+constexpr int kEdgePad = 12, kLongThreads = 128, kLongBatch = 8;
+
+struct LongLine {                                                    // line l of the axis: (outer a, inner b) and its grid offset
+    int a, b;
+    int64_t base;
+};
+
+__device__ inline LongLine long_line(const smb_aug_prefilter_job &jb, int axis, int64_t l) {
+    const int E1 = jb.n1 + 4, E2 = jb.n2 + 4;
+    const int r1 = axis == 2 ? E1 : jb.n2;
+    LongLine ln;
+    ln.a = (int)(l / r1);
+    ln.b = (int)(l % r1);
+    ln.base = axis == 0 ? (int64_t)(ln.a + 2) * E2 + (ln.b + 2)
+                        : (axis == 1 ? (int64_t)ln.a * E1 * E2 + (ln.b + 2) : (int64_t)ln.a * E1 * E2 + (int64_t)ln.b * E2);
+    return ln;
+}
+
+__device__ inline int64_t long_lines(const smb_aug_prefilter_job &jb, int axis) {
+    return axis == 0 ? (int64_t)jb.n1 * jb.n2 : (axis == 1 ? (int64_t)(jb.n0 + 4) * jb.n2 : (int64_t)(jb.n0 + 4) * (jb.n1 + 4));
+}
+
+// c+ at q = 9 (p = -3) from the gained edge value g0 and the first samples of the line, ld(p) for p in [0, n)
+template <class Ld> __device__ inline float long_causal_start(float g0, int n, Ld &&ld) {
+    const float z = kPole;
+    float acc = g0, zi = z;
+    for (int q = 1; q < kEdgePad; ++q) {
+        acc += zi * g0;
+        zi *= z;
+    }
+    for (int p = 0; p < n && zi != 0.f; ++p) {
+        acc += zi * (6.f * ld(p));
+        zi *= z;
+    }
+    float c = acc * z + g0;                                           // q = 0
+    for (int q = 1; q < kEdgePad - 2; ++q) c = g0 + z * c;
+    return c;
+}
+
+// axes 0 and 1: one line per thread, adjacent lanes on adjacent lines (coalesced); kLongBatch loads ahead of the recursion
+__global__ void __launch_bounds__(kLongThreads) prefilter_long_strided_kernel(Jobs<smb_aug_prefilter_job> jobs, int axis) {
+    const smb_aug_prefilter_job jb = jobs.j[blockIdx.y];
+    const int n = axis == 0 ? jb.n0 : jb.n1;
+    if (n <= kAugShortLine) return;                                   // prefilter_kernel's line
+    const int64_t l = (int64_t)blockIdx.x * kLongThreads + threadIdx.x;
+    if (l >= long_lines(jb, axis)) return;
+    const LongLine ln = long_line(jb, axis, l);
+    const int64_t step = axis == 0 ? (int64_t)(jb.n1 + 4) * (jb.n2 + 4) : jb.n2 + 4;
+    float *cf = jb.coef + ln.base + 2 * step;                         // cf[p * step]: grid position p of the line
+    auto ld = [&](int p) -> float {
+        return axis == 0 ? jb.src[((int64_t)p * jb.n1 + ln.a) * jb.n2 + ln.b] : cf[p * step];
+    };
+    const float z = kPole, s0 = ld(0), sl = ld(n - 1), g0 = 6.f * s0, gl = 6.f * sl;
+    float c = long_causal_start(g0, n, ld);
+    for (int p0 = -2; p0 < n + 2; p0 += kLongBatch) {                 // causal: c+ over p = -2 .. n + 1
+        float x[kLongBatch];
+#pragma unroll
+        for (int k = 0; k < kLongBatch; ++k) {
+            const int p = p0 + k;
+            x[k] = p < 0 ? s0 : (p < n ? ld(p) : sl);
+        }
+#pragma unroll
+        for (int k = 0; k < kLongBatch; ++k) {
+            const int p = p0 + k;
+            if (p < n + 2) {
+                c = 6.f * x[k] + z * c;
+                cf[p * step] = c;
+            }
+        }
+    }
+    float tail[kEdgePad - 2];                                         // c+ at p = n + 2 .. n + 11
+#pragma unroll
+    for (int k = 0; k < kEdgePad - 2; ++k) tail[k] = c = gl + z * c;
+    float d = tail[kEdgePad - 3] * (z / (z - 1.f));                   // anticausal
+#pragma unroll
+    for (int k = kEdgePad - 4; k >= 0; --k) d = z * (d - tail[k]);
+    for (int p0 = n + 1; p0 >= -2; p0 -= kLongBatch) {
+        float x[kLongBatch];
+#pragma unroll
+        for (int k = 0; k < kLongBatch; ++k) x[k] = p0 - k >= -2 ? cf[(p0 - k) * step] : 0.f;
+#pragma unroll
+        for (int k = 0; k < kLongBatch; ++k)
+            if (p0 - k >= -2) {
+                d = z * (d - x[k]);
+                cf[(p0 - k) * step] = d;
+            }
+    }
+}
+
+// axis 2 (contiguous lines): a warp stages 32 lines x 32 samples transposed in shared memory, lane t runs the recursion of line t
+__global__ void __launch_bounds__(kLongThreads) prefilter_long_rows_kernel(Jobs<smb_aug_prefilter_job> jobs) {
+    __shared__ float tile[kLongThreads / 32][32][33];
+    const smb_aug_prefilter_job jb = jobs.j[blockIdx.y];
+    const int n = jb.n2, E2 = n + 4;
+    if (n <= kAugShortLine) return;
+    const int lane = threadIdx.x & 31;
+    const int64_t lines = long_lines(jb, 2), l0 = ((int64_t)blockIdx.x * kLongThreads + threadIdx.x) - lane;
+    if (l0 >= lines) return;                                          // the whole warp
+    float(*T)[33] = tile[threadIdx.x >> 5];
+    const bool live = l0 + lane < lines;
+    const int64_t base = live ? long_line(jb, 2, l0 + lane).base : 0;
+    const int nl = lines - l0 < 32 ? (int)(lines - l0) : 32;
+    float *row = jb.coef + base;                                      // row[p + 2]: grid position p of this lane's line
+    const float z = kPole;
+    float c = 0.f, s0 = 0.f, sl = 0.f;
+    if (live) {
+        s0 = row[2];
+        sl = row[n + 1];
+        c = long_causal_start(6.f * s0, n, [&](int p) { return row[p + 2]; });
+    }
+    const float g0 = 6.f * s0, gl = 6.f * sl;
+    for (int e0 = 0; e0 < E2; e0 += 32) {                            // causal, tiles of grid index e = p + 2
+        for (int u = 0; u < nl; ++u) {
+            const int64_t bu = __shfl_sync(0xffffffffu, base, u);
+            const int e = e0 + lane;
+            if (e >= 2 && e < n + 2) T[u][lane] = jb.coef[bu + e];
+        }
+        __syncwarp();
+        if (live)
+            for (int k = 0; k < 32 && e0 + k < E2; ++k) {
+                const int p = e0 + k - 2;
+                c = (p < 0 ? g0 : (p < n ? 6.f * T[lane][k] : gl)) + z * c;
+                T[lane][k] = c;
+            }
+        __syncwarp();
+        for (int u = 0; u < nl; ++u) {
+            const int64_t bu = __shfl_sync(0xffffffffu, base, u);
+            if (e0 + lane < E2) jb.coef[bu + e0 + lane] = T[u][lane];
+        }
+        __syncwarp();
+    }
+    float tail[kEdgePad - 2];
+#pragma unroll
+    for (int k = 0; k < kEdgePad - 2; ++k) tail[k] = c = gl + z * c;
+    float d = tail[kEdgePad - 3] * (z / (z - 1.f));
+#pragma unroll
+    for (int k = kEdgePad - 4; k >= 0; --k) d = z * (d - tail[k]);
+    for (int e0 = (E2 - 1) / 32 * 32; e0 >= 0; e0 -= 32) {            // anticausal, tiles backward
+        for (int u = 0; u < nl; ++u) {
+            const int64_t bu = __shfl_sync(0xffffffffu, base, u);
+            if (e0 + lane < E2) T[u][lane] = jb.coef[bu + e0 + lane];
+        }
+        __syncwarp();
+        if (live)
+            for (int k = (E2 - 1 - e0 < 31 ? E2 - 1 - e0 : 31); k >= 0; --k) {
+                d = z * (d - T[lane][k]);
+                T[lane][k] = d;
+            }
+        __syncwarp();
+        for (int u = 0; u < nl; ++u) {
+            const int64_t bu = __shfl_sync(0xffffffffu, base, u);
+            if (e0 + lane < E2) jb.coef[bu + e0 + lane] = T[u][lane];
+        }
+        __syncwarp();
     }
 }
 
@@ -477,22 +641,39 @@ cudaError_t aug_crop_launch(const smb_aug_crop_args &a, cudaStream_t st) {
 }
 
 cudaError_t aug_prefilter_launch(const smb_aug_prefilter_job *jobs, int n, cudaStream_t st) {
+    // per axis, each job's lines go to the staged kernel (n <= kAugShortLine) or to the streaming one (longer, edge boundary)
     return for_chunks(jobs, n, [&](const Jobs<smb_aug_prefilter_job> &js, int) {
-        int maxn = 0;
-        int64_t maxlines[3] = {0, 0, 0};
-        for (int q = 0; q < js.n; ++q) {
-            const smb_aug_prefilter_job &j = js.j[q];
-            const int m = j.n0 > j.n1 ? (j.n0 > j.n2 ? j.n0 : j.n2) : (j.n1 > j.n2 ? j.n1 : j.n2);
-            maxn = m > maxn ? m : maxn;
-            const int64_t l[3] = {(int64_t)j.n1 * j.n2, (int64_t)(j.n0 + 4) * j.n2, (int64_t)(j.n0 + 4) * (j.n1 + 4)};
-            for (int d = 0; d < 3; ++d) maxlines[d] = l[d] > maxlines[d] ? l[d] : maxlines[d];
-        }
-        const size_t smem = sizeof(float) * 33 * (size_t)(maxn + 24);
         for (int axis = 0; axis < 3; ++axis) {
-            prefilter_kernel<<<dim3((unsigned)((maxlines[axis] + 31) / 32), js.n), 32, smem, st>>>(js, axis);
-            count_launch();
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return e;
+            int maxn = 0;
+            int64_t short_lines = 0, long_lines = 0;
+            for (int q = 0; q < js.n; ++q) {
+                const smb_aug_prefilter_job &j = js.j[q];
+                const int na = axis == 0 ? j.n0 : (axis == 1 ? j.n1 : j.n2);
+                const int64_t l = axis == 0 ? (int64_t)j.n1 * j.n2 : (int64_t)(j.n0 + 4) * (axis == 1 ? j.n2 : j.n1 + 4);
+                if (na <= kAugShortLine) {
+                    maxn = na > maxn ? na : maxn;
+                    short_lines = l > short_lines ? l : short_lines;
+                } else {
+                    long_lines = l > long_lines ? l : long_lines;
+                }
+            }
+            if (short_lines) {
+                const size_t smem = sizeof(float) * 33 * (size_t)(maxn + 24);
+                prefilter_kernel<<<dim3((unsigned)((short_lines + 31) / 32), js.n), 32, smem, st>>>(js, axis);
+                count_launch();
+                cudaError_t e = cudaGetLastError();
+                if (e != cudaSuccess) return e;
+            }
+            if (long_lines) {
+                const dim3 grid((unsigned)((long_lines + kLongThreads - 1) / kLongThreads), js.n);
+                if (axis == 2)
+                    prefilter_long_rows_kernel<<<grid, kLongThreads, 0, st>>>(js);
+                else
+                    prefilter_long_strided_kernel<<<grid, kLongThreads, 0, st>>>(js, axis);
+                count_launch();
+                cudaError_t e = cudaGetLastError();
+                if (e != cudaSuccess) return e;
+            }
         }
         return cudaSuccess;
     });

@@ -498,9 +498,12 @@ SMB_API int smb_aug_prefilter(const smb_aug_prefilter_job *jobs, int32_t n_jobs,
     for (int q = 0; q < n_jobs; ++q) {
         const smb_aug_prefilter_job &j = jobs[q];
         if (!j.src || !j.coef) return fail(SMB_EINVAL, "smb_aug_prefilter: job %d needs src and coef", q);
-        if (j.n0 < 4 || j.n1 < 4 || j.n2 < 4 || j.n0 > smb::kAugMaxAxis || j.n1 > smb::kAugMaxAxis || j.n2 > smb::kAugMaxAxis)
-            return fail(SMB_EUNSUPPORTED, "smb_aug_prefilter: job %d: axes must be 4..%d samples", q, smb::kAugMaxAxis);
+        if (j.n0 < 4 || j.n1 < 4 || j.n2 < 4) return fail(SMB_EUNSUPPORTED, "smb_aug_prefilter: job %d: axes must be at least 4 samples", q);
         if (j.boundary != SMB_AUG_MIRROR && j.boundary != SMB_AUG_EDGE) return fail(SMB_EINVAL, "smb_aug_prefilter: job %d: bad boundary", q);
+        if (j.boundary == SMB_AUG_MIRROR && (j.n0 > smb::kAugMaxAxis || j.n1 > smb::kAugMaxAxis || j.n2 > smb::kAugMaxAxis))
+            return fail(SMB_EUNSUPPORTED, "smb_aug_prefilter: job %d: mirror-boundary axes must be 4..%d samples", q, smb::kAugMaxAxis);
+        if ((int64_t)(j.n0 + 4) * (j.n1 + 4) * (j.n2 + 4) > INT32_MAX)
+            return fail(SMB_EUNSUPPORTED, "smb_aug_prefilter: job %d: the coefficient grid is limited to 2^31 - 1 voxels", q);
     }
     cudaError_t e = smb::aug_prefilter_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_aug_prefilter");
@@ -512,8 +515,11 @@ SMB_API int smb_aug_resample(const smb_aug_resample_job *jobs, int32_t n_jobs, v
     for (int q = 0; q < n_jobs; ++q) {
         const smb_aug_resample_job &j = jobs[q];
         if (!j.src || !j.dst) return fail(SMB_EINVAL, "smb_aug_resample: job %d needs src and dst", q);
-        if (!aug_axis_ok(j.n0) || !aug_axis_ok(j.n1) || !aug_axis_ok(j.n2) || !aug_axis_ok(j.m0) || !aug_axis_ok(j.m1) || !aug_axis_ok(j.m2))
-            return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: axes must be 1..%d samples", q, smb::kAugMaxAxis);
+        if (j.n0 < 1 || j.n1 < 1 || j.n2 < 1 || j.m0 < 1 || j.m1 < 1 || j.m2 < 1)
+            return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: axes must be positive", q);
+        const int b = j.order == 3 ? 4 : 0;                           // order 3 reads the border-extended coefficient grid
+        if ((int64_t)(j.n0 + b) * (j.n1 + b) * (j.n2 + b) > INT32_MAX || (int64_t)j.m0 * j.m1 * j.m2 > INT32_MAX)
+            return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: source and output are limited to 2^31 - 1 voxels", q);
         if (j.order != 0 && j.order != 1 && j.order != 3) return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: order %d (0, 1, 3)", q, j.order);
         if (j.map != SMB_AUG_AFFINE && j.map != SMB_AUG_ZOOM) return fail(SMB_EINVAL, "smb_aug_resample: job %d: bad map", q);
         if (j.order == 1 && (j.map != SMB_AUG_AFFINE || j.clip)) return fail(SMB_EUNSUPPORTED, "smb_aug_resample: job %d: labels take an affine map, no clip", q);
@@ -717,6 +723,16 @@ SMB_API int smb_prep_normalize(const smb_prep_norm_job *jobs, int32_t n_jobs, vo
             return fail(SMB_EINVAL, "smb_prep_normalize: job %d: src, dst, stats, moments, n > 0 required", q);
     cudaError_t e = smb::prep_normalize_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_prep_normalize");
+    return SMB_OK;
+}
+
+SMB_API int smb_prep_ct_normalize(const smb_prep_ct_norm_job *jobs, int32_t n_jobs, void *cuda_stream) {
+    if (n_jobs < 0 || (n_jobs > 0 && !jobs)) return fail(SMB_EINVAL, "smb_prep_ct_normalize: bad job list");
+    for (int q = 0; q < n_jobs; ++q)
+        if (!jobs[q].src || !jobs[q].dst || jobs[q].n <= 0)
+            return fail(SMB_EINVAL, "smb_prep_ct_normalize: job %d: src, dst, n > 0 required", q);
+    cudaError_t e = smb::prep_ct_normalize_launch(jobs, n_jobs, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_prep_ct_normalize");
     return SMB_OK;
 }
 

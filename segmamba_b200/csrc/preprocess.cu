@@ -126,6 +126,19 @@ __global__ void __launch_bounds__(kThreads) normalize_kernel(Jobs<smb_prep_norm_
         jb.dst[v] = (float)(((double)jb.src[v] - mean) / div);
 }
 
+// ---- CT normalisation -----------------------------------------------------------------------------------------------------------
+// numpy's clip (maximum, then minimum; a NaN passes through, -0 stays -0) and two fp32 operations: a subtraction and an IEEE
+// division cannot contract into an FMA, so the result is bit-equal to numpy's float32 arithmetic
+__global__ void __launch_bounds__(kThreads) ct_normalize_kernel(Jobs<smb_prep_ct_norm_job> jobs) {
+    const smb_prep_ct_norm_job jb = jobs.j[blockIdx.y];
+    for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < jb.n; v += (int64_t)gridDim.x * blockDim.x) {
+        float x = jb.src[v];
+        x = x < jb.lo ? jb.lo : x;
+        x = x > jb.hi ? jb.hi : x;
+        jb.dst[v] = (x - jb.mean) / jb.div;
+    }
+}
+
 // ---- order-1 label resize -------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads) label_resize_kernel(smb_prep_label_resize_args a) {
     const int n[3] = {a.n0, a.n1, a.n2};
@@ -324,6 +337,14 @@ cudaError_t prep_crop_launch(const smb_prep_crop_args &a, cudaStream_t st) {
 cudaError_t prep_normalize_launch(const smb_prep_norm_job *jobs, int n, cudaStream_t st) {
     return for_chunks(jobs, n, [&](const Jobs<smb_prep_norm_job> &js) {
         normalize_kernel<<<dim3(grid_for(max_n(js), kThreads, js.n), js.n), kThreads, 0, st>>>(js);
+        count_launch();
+        return cudaGetLastError();
+    });
+}
+
+cudaError_t prep_ct_normalize_launch(const smb_prep_ct_norm_job *jobs, int n, cudaStream_t st) {
+    return for_chunks(jobs, n, [&](const Jobs<smb_prep_ct_norm_job> &js) {
+        ct_normalize_kernel<<<dim3(grid_for(max_n(js), kThreads, js.n), js.n), kThreads, 0, st>>>(js);
         count_launch();
         return cudaGetLastError();
     });

@@ -7,6 +7,8 @@ MultiModalityPreprocessor.read_data's foreground intensities and DefaultPreproce
     to it, seg 0 outside the mask set to nonzero_label (without a seg: 0 inside, nonzero_label outside, int8).
   * zscore: ZScoreNormalization(use_mask_for_norm=False) per channel over the whole box, divisor max(std, 1e-8); mean and std
     are fp64 from an ordered reduction (smb_aug_stats), so the result is deterministic.
+  * ct_normalize: CTNormalization per channel from the dataset's foreground statistics (plan.plan_dataset), clip to the
+    0.5 / 99.5 percentiles then (x - mean) / max(std, 1e-8), in fp32 bit-equal to numpy.
   * compute_new_shape: the reference's, with Python round.
   * resample_case: skimage resize(order=3, mode='edge', anti_aliasing=False) of every channel, clipped to its range
     (smb_aug_stats + smb_aug_prefilter + smb_aug_resample, augment.py's low-resolution path), and batchgenerators
@@ -14,13 +16,13 @@ MultiModalityPreprocessor.read_data's foreground intensities and DefaultPreproce
   * sample_foreground_locations / foreground_intensities: the reference's RandomState(seed) draws, made on the host from
     counts read back from the device (choice(n, ...) depends only on n), over indices compacted on the device in raster
     order; the device gathers the drawn rows and intensities.
-  * preprocess_case: all of it in the reference's order, returning (data, seg, properties).
+  * preprocess_case: all of it in the reference's order, returning (data, seg, properties); normalization="ct" runs the
+    DefaultPreprocessor of the reference's CT pipelines instead of the z-score.
 
 Bounds: labels must be integers in [0, 127] (the reference switches to int16 above 127; here that raises ValueError), volumes
-below 2^31 voxels, and a resampled case needs crop axes of 4..256 voxels and target axes of 1..256 voxels (the cubic resize of
-augment.cu stages whole lines in shared memory).
+below 2^31 voxels, and a resampled case needs crop axes of at least 4 voxels.
 
-nonzero_mask, zscore and resample_case never synchronise with the host.  Everything the host needs goes through `_readback`;
+nonzero_mask, zscore, ct_normalize and resample_case never synchronise with the host.  Everything the host needs goes through `_readback`;
 preprocess_case makes exactly READBACKS_PER_CASE (3) of them: the mask record (bbox, foreground count, NaN and label checks),
 the label counts, and the drawn rows with the intensity samples and statistics.
 """
@@ -36,11 +38,10 @@ from . import _lib
 from . import augment as A
 from .predict import fill_holes
 
-__all__ = ["nonzero_mask", "crop_to_nonzero", "zscore", "compute_new_shape", "resample_case", "sample_foreground_locations",
+__all__ = ["nonzero_mask", "crop_to_nonzero", "zscore", "ct_normalize", "compute_new_shape", "resample_case", "sample_foreground_locations",
            "foreground_intensities", "preprocess_case", "READBACKS_PER_CASE"]
 
 READBACKS_PER_CASE = 3
-MAX_RESAMPLE_AXIS = 256          # kAugMaxAxis of csrc/aug_internal.h: the prefilter stages a whole line in shared memory
 _readbacks = 0                   # device-to-host synchronisations made by _readback (tests count them)
 
 
@@ -163,6 +164,30 @@ def zscore(data: torch.Tensor):
     return out, mom
 
 
+_CT_KEYS = ("mean", "std", "percentile_00_5", "percentile_99_5")
+
+
+def ct_normalize(data: torch.Tensor, intensity_properties) -> torch.Tensor:
+    """(C, D, H, W) fp32: CTNormalization(use_mask_for_norm=False) of every channel with intensity_properties[str(c)] (a dict
+    with mean, std, percentile_00_5 and percentile_99_5, as plan.plan_dataset or the reference's data_analysis_result.txt give
+    them): clip to [percentile_00_5, percentile_99_5], then (x - mean) / max(std, 1e-8), all in fp32 as numpy computes it for
+    a float32 image.  Raises ValueError for a missing channel or key.  No synchronisation."""
+    data = _data(data)
+    C, n = data.shape[0], data[0].numel()
+    f = np.float32
+    jobs = []
+    out = torch.empty_like(data)
+    for c in range(C):
+        try:
+            p = intensity_properties[str(c)]
+            mean, std, lo, hi = (p[k] for k in _CT_KEYS)
+        except (KeyError, IndexError, TypeError) as e:
+            raise ValueError(f"intensity_properties needs channel '{c}' with {', '.join(_CT_KEYS)}: {e!r}") from None
+        jobs.append(_lib.PrepCtNormJob(data[c].data_ptr(), out[c].data_ptr(), n, f(lo), f(hi), f(mean), f(max(std, 1e-8))))
+    A._run("smb_prep_ct_normalize", _lib.PrepCtNormJob, jobs, data.device)
+    return out
+
+
 def compute_new_shape(old_shape, old_spacing, new_spacing) -> np.ndarray:
     """the reference's compute_new_shape: int(round(old_spacing / new_spacing * old_shape)) per axis"""
     assert len(old_spacing) == len(old_shape)
@@ -174,7 +199,8 @@ def resample_case(data: torch.Tensor, seg: torch.Tensor | None, new_shape):
     """(data (C, *new_shape) fp32, seg (1, *new_shape) int8 or None): resample_data_or_seg_to_shape with
     force_separate_z=False -- skimage resize(order=3, mode='edge', anti_aliasing=False) of each channel clipped to its range,
     resize_segmentation(order=1) of the labels.  The inputs come back unchanged when the shape does not change.  Raises
-    ValueError outside the resize bounds.  No synchronisation."""
+    ValueError for a source axis below 4 voxels, an empty target axis or a volume of 2^31 voxels or more.  No
+    synchronisation."""
     _lib.require_cuda(data, seg)
     new_shape = tuple(int(v) for v in new_shape)
     src = tuple(data.shape[1:])
@@ -182,9 +208,11 @@ def resample_case(data: torch.Tensor, seg: torch.Tensor | None, new_shape):
         raise ValueError(f"data must be (C, D, H, W) and new_shape three axes, got {tuple(data.shape)} and {new_shape}")
     if new_shape == src:
         return data, seg
-    if min(src) < 4 or max(src) > MAX_RESAMPLE_AXIS or min(new_shape) < 1 or max(new_shape) > MAX_RESAMPLE_AXIS:
-        raise ValueError(f"resampling {src} -> {new_shape}: source axes must be 4..{MAX_RESAMPLE_AXIS} voxels and target axes "
-                         f"1..{MAX_RESAMPLE_AXIS}")
+    if min(src) < 4 or min(new_shape) < 1:
+        raise ValueError(f"resampling {src} -> {new_shape}: source axes need at least 4 voxels and target axes at least 1")
+    if math.prod(v + 4 for v in src) >= 2 ** 31 or math.prod(new_shape) >= 2 ** 31:
+        raise ValueError(f"resampling {src} -> {new_shape}: source (with a 2-voxel border) and target are limited to 2^31 - 1 "
+                         f"voxels")
     data = data.to(torch.float32).contiguous()
     C, dev = data.shape[0], data.device
     st = _stats(data)
@@ -389,18 +417,25 @@ def foreground_intensities(data: torch.Tensor, seg: torch.Tensor, seed: int = 12
 
 
 def preprocess_case(data: torch.Tensor, seg: torch.Tensor | None = None, spacing=(1.0, 1.0, 1.0), target_spacing=(1, 1, 1),
-                    all_labels=(1, 2, 3), name=None):
+                    all_labels=(1, 2, 3), name=None, normalization: str = "zscore", intensity_properties=None):
     """(data (C, d, h, w) fp32, seg (1, d, h, w) int8, properties) of one raw case, as the reference's read_data +
-    run_case_npy with ZScoreNormalization, on the device.
+    run_case_npy on the device: MultiModalityPreprocessor's (ZScoreNormalization, normalization="zscore") or
+    DefaultPreprocessor's (CTNormalization, normalization="ct", with the dataset's intensity_properties).
 
     data      CUDA (C, D, H, W); other dtypes are converted to fp32
     seg       CUDA (1, D, H, W) or (D, H, W) integer labels in [0, 127] (integer or integral float dtype), or None
     spacing   SimpleITK (x, y, z) order, as properties["spacing"]
     target_spacing  the reference's output_spacing (array order)
     all_labels      labels or regions (tuples / lists of labels) for class_locations
+    intensity_properties  normalization="ct" only: {"0": {mean, std, percentile_00_5, percentile_99_5}, ...} per channel,
+                    plan.plan_dataset(...)["intensity_statistics_per_channel"]
 
     The output data and seg stay on the device; class_locations are numpy int64 (k, 4) arrays.  Makes exactly
     READBACKS_PER_CASE (3) synchronisations: the mask record, the label counts, the drawn rows and intensity statistics."""
+    if normalization not in ("zscore", "ct"):
+        raise ValueError(f"normalization must be 'zscore' or 'ct', got {normalization!r}")
+    if normalization == "ct" and intensity_properties is None:
+        raise ValueError("normalization='ct' needs the dataset's intensity_properties")
     data = _data(data)
     seg_in = _seg(seg, data.shape[1:])
     C, D, H, W = data.shape
@@ -414,7 +449,7 @@ def preprocess_case(data: torch.Tensor, seg: torch.Tensor | None = None, spacing
     crop_shape = tuple(crop.shape[1:])
     original_spacing_trans = list(spacing)[::-1]
     new_shape = compute_new_shape(crop_shape, original_spacing_trans, target_spacing)
-    norm, _ = zscore(crop)
+    norm = ct_normalize(crop, intensity_properties) if normalization == "ct" else zscore(crop)[0]
     out, oseg = resample_case(norm, cseg, new_shape)
     classes = list(all_labels)
     comp = _Compaction(oseg, [_class_labels(c) for c in classes])
