@@ -544,6 +544,73 @@ typedef struct smb_metric_select_args {
 
 SMB_API int smb_metric_select(const smb_metric_select_args *args, void *cuda_stream);
 
+/* Per-class evaluation (metrics.class_metrics): class k is the set of voxels whose label is classes[k], for up to 255 disjoint
+ * classes.  smb_metric_region_bits with lut[classes[k]] = k + 1 writes the class maps (0: no class).  Then
+ *   smb_metric_class_count  per (sample, class) counts, border-voxel counts and the bounding box of the border voxels of P and
+ *                           G, and the two border maps
+ *   smb_metric_class_edt    the EDT of smb_metric_edt over a table of jobs in device memory, each restricted to its box
+ *   smb_metric_class_reduce per pool: the maximum, the q-th percentile and the mean distance of each direction
+ * The host reads the count record back in between to plan the jobs and size the workspace. */
+#define SMB_METRIC_I16 5
+#define SMB_METRIC_MAX_CLASSES 255
+#define SMB_METRIC_CLASS_NREC 11      /* int64 per (sample, class), see smb_metric_class_count */
+
+/* record[(b * classes + k) * SMB_METRIC_CLASS_NREC + i] for class value k + 1 of the class maps (the caller zeroes it):
+ * i = 0..4: |P|, |G|, |P and G|, |border P|, |border G|;  i = 5..7: d - z_lo, h - y_lo, w - x_lo and i = 8..10: z_hi + 1,
+ * y_hi + 1, x_hi + 1 of the inclusive bounding box of the border voxels of P and G (all 0 when there are none).  A border voxel
+ * has a class and a 6-neighbour of another class or outside the volume.  The border maps get the voxel's class value at border
+ * voxels, 0 elsewhere. */
+typedef struct smb_metric_class_count_args {
+    const void *pred, *target;  /* (batch, d, h, w) uint8 class maps */
+    void *pred_border, *target_border;
+    int64_t *record;
+    int32_t batch, classes, d, h, w;
+} smb_metric_class_count_args;
+
+SMB_API int smb_metric_class_count(const smb_metric_class_count_args *args, void *cuda_stream);
+
+/* One EDT job: a box of bd x bh x bw voxels of one sample's border maps.  Voxel v is a source where (src[v] & src_mask) ==
+ * src_val and a target where (tgt[v] & tgt_mask) == tgt_val.  The distance from every source voxel to the nearest target voxel
+ * (as smb_metric_edt) is appended at pool[(*fill)++]; lines, if not NULL, gets per line of axis 1 (z * bw + x) the sum, in
+ * order of y, and the maximum of its source distances.  feat: bd * bh * bw int32 of workspace. */
+typedef struct smb_metric_edt_job {
+    const void *src, *tgt;      /* the box origin in the maps, which have the row and slice strides of the args */
+    int32_t *feat;
+    double *pool;
+    int64_t *fill;
+    double *lines;              /* bd * bw (sum, max) pairs */
+    int32_t bd, bh, bw, src_mask, src_val, tgt_mask, tgt_val;
+} smb_metric_edt_job;
+
+/* Every job has bd <= max_d, bh <= max_h <= SMB_METRIC_MAX_AXIS, bw <= max_w <= SMB_METRIC_MAX_AXIS, bd * bh * bw < 2^31. */
+typedef struct smb_metric_class_edt_args {
+    const smb_metric_edt_job *jobs;   /* njobs, in device memory */
+    int64_t row_stride, slice_stride;  /* of the maps, in voxels */
+    int32_t njobs, max_d, max_h, max_w;
+    double s0, s1, s2;
+} smb_metric_class_edt_args;
+
+SMB_API int smb_metric_class_edt(const smb_metric_class_edt_args *args, void *cuda_stream);
+
+/* One (sample, class) pair: dist holds the n0 distances from P's border and the n1 from G's border (any order); lines holds
+ * lines0 then lines1 (sum, max) pairs of the two directions.  n0 and n1 must be positive. */
+typedef struct smb_metric_pool {
+    const double *dist, *lines;
+    int64_t n0, n1;
+    int32_t lines0, lines1;
+} smb_metric_pool;
+
+/* out[p * 4 + 0..3] = hd (the maximum), numpy.percentile(dist, 100 * frac) ('linear'), asd = sum0 / n0 and assd =
+ * (sum0 / n0 + sum1 / n1) / 2 of pool p; each sum adds the line sums in a fixed order. */
+typedef struct smb_metric_class_reduce_args {
+    const smb_metric_pool *pools;     /* npools, in device memory */
+    double *out;
+    int32_t npools;
+    double frac;
+} smb_metric_class_reduce_args;
+
+SMB_API int smb_metric_class_reduce(const smb_metric_class_reduce_args *args, void *cuda_stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Case prediction on the GPU (segmamba_b200/predict.py): the steps of the reference's Predictor after the sliding window,
  * plus exact 6-connected component post-processing.  All calls enqueue on `cuda_stream`, allocate nothing, never synchronise

@@ -181,8 +181,32 @@ class MetricSelectArgs(ctypes.Structure):
                 + [(n, _i32) for n in ("batch", "regions")] + [("frac", _f64)])
 
 
+class MetricClassCountArgs(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("pred", "target", "pred_border", "target_border", "record")]
+                + [(n, _i32) for n in ("batch", "classes", "d", "h", "w")])
+
+
+class MetricEdtJob(ctypes.Structure):
+    _fields_ = ([(n, _vp) for n in ("src", "tgt", "feat", "pool", "fill", "lines")]
+                + [(n, _i32) for n in ("bd", "bh", "bw", "src_mask", "src_val", "tgt_mask", "tgt_val")])
+
+
+class MetricClassEdtArgs(ctypes.Structure):
+    _fields_ = ([("jobs", _vp)] + [(n, _i64) for n in ("row_stride", "slice_stride")]
+                + [(n, _i32) for n in ("njobs", "max_d", "max_h", "max_w")] + [(n, _f64) for n in ("s0", "s1", "s2")])
+
+
+class MetricPool(ctypes.Structure):
+    _fields_ = [("dist", _vp), ("lines", _vp), ("n0", _i64), ("n1", _i64), ("lines0", _i32), ("lines1", _i32)]
+
+
+class MetricClassReduceArgs(ctypes.Structure):
+    _fields_ = [("pools", _vp), ("out", _vp), ("npools", _i32), ("frac", _f64)]
+
+
 METRIC_MAX_REGIONS, METRIC_MAX_AXIS, METRIC_NCOUNTS = 8, 768, 8
-METRIC_I8, METRIC_U8, METRIC_I32, METRIC_I64, METRIC_LOGITS = 0, 1, 2, 3, 4
+METRIC_I8, METRIC_U8, METRIC_I32, METRIC_I64, METRIC_LOGITS, METRIC_I16 = 0, 1, 2, 3, 4, 5
+METRIC_MAX_CLASSES, METRIC_CLASS_NREC = 255, 11
 
 
 # case prediction (include/segmamba_b200.h, "Case prediction on the GPU")
@@ -273,6 +297,9 @@ EXPORTS = {
     "smb_metric_count": (ctypes.c_int, [ctypes.POINTER(MetricCountArgs), _vp]),
     "smb_metric_edt": (ctypes.c_int, [ctypes.POINTER(MetricEdtArgs), _vp]),
     "smb_metric_select": (ctypes.c_int, [ctypes.POINTER(MetricSelectArgs), _vp]),
+    "smb_metric_class_count": (ctypes.c_int, [ctypes.POINTER(MetricClassCountArgs), _vp]),
+    "smb_metric_class_edt": (ctypes.c_int, [ctypes.POINTER(MetricClassEdtArgs), _vp]),
+    "smb_metric_class_reduce": (ctypes.c_int, [ctypes.POINTER(MetricClassReduceArgs), _vp]),
     "smb_pred_restore": (ctypes.c_int, [ctypes.POINTER(PredRestoreArgs), _vp]),
     "smb_pred_cc_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
     "smb_pred_cc": (ctypes.c_int, [ctypes.POINTER(PredCcArgs), _vp]),

@@ -597,7 +597,7 @@ SMB_API int smb_metric_region_bits(const smb_metric_bits_args *a, void *cuda_str
     if (!a->src || !a->bits) return fail(SMB_EINVAL, "smb_metric_region_bits: src and bits are required");
     if (a->batch <= 0 || a->batch > 65535 || a->voxels <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: batch (1..65535) and voxels must be positive");
     if (a->sample_stride < 0 || a->voxel_stride <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: bad strides");
-    if (a->kind < SMB_METRIC_I8 || a->kind > SMB_METRIC_LOGITS) return fail(SMB_EINVAL, "smb_metric_region_bits: bad kind %d", a->kind);
+    if (a->kind < SMB_METRIC_I8 || a->kind > SMB_METRIC_I16) return fail(SMB_EINVAL, "smb_metric_region_bits: bad kind %d", a->kind);
     if (a->kind == SMB_METRIC_LOGITS) {
         if (a->dtype < SMB_F32 || a->dtype > SMB_BF16) return fail(SMB_EINVAL, "smb_metric_region_bits: bad dtype %d", a->dtype);
         if (a->classes <= 0 || a->class_stride <= 0) return fail(SMB_EINVAL, "smb_metric_region_bits: logits need classes and class_stride > 0");
@@ -641,6 +641,45 @@ SMB_API int smb_metric_select(const smb_metric_select_args *a, void *cuda_stream
     if (!(a->frac >= 0.0 && a->frac <= 1.0)) return fail(SMB_EINVAL, "smb_metric_select: frac must be in [0, 1]");
     cudaError_t e = smb::metric_select_launch(*a, (cudaStream_t)cuda_stream);
     if (e != cudaSuccess) return cuda_fail(e, "smb_metric_select");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_class_count(const smb_metric_class_count_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_class_count: null args");
+    if (a->batch <= 0 || a->batch > 65535 || a->d <= 0 || a->h <= 0 || a->w <= 0)
+        return fail(SMB_EINVAL, "smb_metric_class_count: batch (1..65535) and axes must be positive");
+    if (a->classes <= 0 || a->classes > SMB_METRIC_MAX_CLASSES) return fail(SMB_EINVAL, "smb_metric_class_count: classes must be 1..%d", SMB_METRIC_MAX_CLASSES);
+    if ((int64_t)a->d * a->h * a->w > INT32_MAX) return fail(SMB_EUNSUPPORTED, "smb_metric_class_count: volumes are limited to 2^31 - 1 voxels");
+    if (!a->pred || !a->target || !a->pred_border || !a->target_border || !a->record)
+        return fail(SMB_EINVAL, "smb_metric_class_count: pred, target, pred_border, target_border, record are required");
+    cudaError_t e = smb::metric_class_count_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_class_count");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_class_edt(const smb_metric_class_edt_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_class_edt: null args");
+    if (!a->jobs) return fail(SMB_EINVAL, "smb_metric_class_edt: jobs is required");
+    if (a->njobs <= 0 || a->njobs > 65535) return fail(SMB_EUNSUPPORTED, "smb_metric_class_edt: njobs must be 1..65535");
+    if (a->max_d <= 0 || a->max_h <= 0 || a->max_w <= 0) return fail(SMB_EINVAL, "smb_metric_class_edt: box bounds must be positive");
+    if (a->max_h > SMB_METRIC_MAX_AXIS || a->max_w > SMB_METRIC_MAX_AXIS)
+        return fail(SMB_EUNSUPPORTED, "smb_metric_class_edt: box axes 1 and 2 are limited to %d voxels", SMB_METRIC_MAX_AXIS);
+    if (a->row_stride < a->max_w || a->slice_stride < a->row_stride * a->max_h)
+        return fail(SMB_EINVAL, "smb_metric_class_edt: the map strides must cover the box bounds");
+    if (!(a->s0 > 0.0 && a->s1 > 0.0 && a->s2 > 0.0) || !std::isfinite(a->s0 * a->s1 * a->s2))
+        return fail(SMB_EINVAL, "smb_metric_class_edt: spacing must be positive and finite");
+    cudaError_t e = smb::metric_class_edt_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_class_edt");
+    return SMB_OK;
+}
+
+SMB_API int smb_metric_class_reduce(const smb_metric_class_reduce_args *a, void *cuda_stream) {
+    if (!a) return fail(SMB_EINVAL, "smb_metric_class_reduce: null args");
+    if (!a->pools || !a->out) return fail(SMB_EINVAL, "smb_metric_class_reduce: pools and out are required");
+    if (a->npools <= 0) return fail(SMB_EINVAL, "smb_metric_class_reduce: npools must be positive");
+    if (!(a->frac >= 0.0 && a->frac <= 1.0)) return fail(SMB_EINVAL, "smb_metric_class_reduce: frac must be in [0, 1]");
+    cudaError_t e = smb::metric_class_reduce_launch(*a, (cudaStream_t)cuda_stream);
+    if (e != cudaSuccess) return cuda_fail(e, "smb_metric_class_reduce");
     return SMB_OK;
 }
 

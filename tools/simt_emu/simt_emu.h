@@ -213,6 +213,11 @@ inline int atomicMin(int *addr, int val) {
     while (val < old && !__atomic_compare_exchange_n(addr, &old, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
     return old;
 }
+inline unsigned atomicMax(unsigned *addr, unsigned val) {
+    unsigned old = __atomic_load_n(addr, __ATOMIC_RELAXED);
+    while (val > old && !__atomic_compare_exchange_n(addr, &old, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+    return old;
+}
 inline unsigned long long atomicMax(unsigned long long *addr, unsigned long long val) {
     unsigned long long old = __atomic_load_n(addr, __ATOMIC_RELAXED);
     while (val > old && !__atomic_compare_exchange_n(addr, &old, val, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
