@@ -143,8 +143,13 @@ __global__ void __launch_bounds__(kConvThreads) conv1d_bwd_kernel(const ConvP p)
 #pragma unroll
         for (int k = 0; k < 4; ++k) acc = fmaf(w4[k], gh[i + 3 - k], acc);
         dxv[i] = acc;
+        // causal_conv1d_bwd.cu:216-222; a tap over the zero padding before position 0 is skipped rather than multiplied by 0,
+        // so a non-finite g-hat at the first positions reaches only the taps that read input, as in the reference
 #pragma unroll
-        for (int k = 0; k < 4; ++k) dw[k] = fmaf(x[i + k], gh[i], dw[k]);   // causal_conv1d_bwd.cu:216-222
+        for (int k = 0; k < 4; ++k) {
+            const float t = x[i + k] * gh[i];
+            dw[k] += (j + i + k >= 3) ? t : 0.f;
+        }
         db += gh[i];
     }
     store_run8<T>(dxr, j, L, p.reverse, dxv);

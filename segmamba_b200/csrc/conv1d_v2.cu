@@ -142,8 +142,13 @@ __global__ void __launch_bounds__(kConv2Threads) conv1d_bwd16_kernel(const ConvP
 #pragma unroll
         for (int k = 0; k < 4; ++k) acc = fmaf(w4[k], gh[i + 3 - k], acc);     // dx[j+i] = sum_k w4[k] ghat[j+i+3-k]
         dxv[i] = acc;
+        // x[i + k] is position j + i + k - 3: a tap over the zero padding before position 0 is selected away, not multiplied
+        // by 0, so a non-finite g-hat at the first positions reaches only the taps that read input, as in the reference
 #pragma unroll
-        for (int k = 0; k < 4; ++k) dw[k] = fmaf(x[i + k], gh[i], dw[k]);
+        for (int k = 0; k < 4; ++k) {
+            const float t = x[i + k] * gh[i];
+            dw[k] += (j + i + k >= 3) ? t : 0.f;
+        }
         db += gh[i];
     }
     store_run16<T>(dxr, j, L, p.reverse, dxv);

@@ -44,15 +44,19 @@ constexpr int kNormThreads = 256;
 #define SMB_IN_U_BWD2 1
 #endif
 
+// Non-finite semantics are torch's: ReLU is threshold(v, 0, 0), so NaN passes through it, and its backward
+// (threshold_backward) selects rather than multiplies -- g passes where v is NaN and is dropped, even if non-finite, where
+// v <= 0.  LeakyReLU's backward multiplies (g * slope), as leaky_relu_backward does.
 __device__ __forceinline__ float act_fwd(float v, int act, float slope) {
-    if (act == 1) return v > 0.f ? v : 0.f;
+    if (act == 1) return v <= 0.f ? 0.f : v;
     if (act == 2) return v > 0.f ? v : slope * v;
     return v;
 }
-__device__ __forceinline__ float act_grad(float v, int act, float slope) {
-    if (act == 1) return v > 0.f ? 1.f : 0.f;
-    if (act == 2) return v > 0.f ? 1.f : slope;
-    return 1.f;
+// g * act'(v), for the incoming gradient g and the pre-activation v
+__device__ __forceinline__ float act_bwd(float g, float v, int act, float slope) {
+    if (act == 1) return v <= 0.f ? 0.f : g;
+    if (act == 2) return v > 0.f ? g : g * slope;
+    return g;
 }
 
 // Build-time knob (tools/build_variants.py in_rev): the apply passes walk their row range from the top down.  The statistics pass
@@ -327,7 +331,7 @@ __global__ void __launch_bounds__(kNormThreads, (MODE2 == 0 ? SMB_IN_BWD_MINB0 :
                         const float xh = (a[k][v] - mu[v]) * rs[v];
                         float pre = xh, xh2 = 0.f;
                         if (MODE2) { xh2 = (a2[k][v] - mu2[v]) * rs2[v]; pre += xh2; }
-                        const float gg = g[k][v] * act_grad(pre, p.act, p.slope);
+                        const float gg = act_bwd(g[k][v], pre, p.act, p.slope);
                         sg[v] += gg;
                         sgx[v] = fmaf(gg, xh, sgx[v]);
                         if (MODE2 == 2) sgx2[v] = fmaf(gg, xh2, sgx2[v]);
@@ -430,7 +434,7 @@ __global__ void __launch_bounds__(kNormThreads, (MODE2 == 0 ? SMB_IN_BWD_MINB0 :
                     const float xh = (a[k][v] - mu[v]) * rs[v];
                     float pre = xh, xh2 = 0.f;
                     if (MODE2) { xh2 = (a2[k][v] - mu2[v]) * rs2[v]; pre += xh2; }
-                    const float gg = g[k][v] * act_grad(pre, p.act, p.slope);
+                    const float gg = act_bwd(g[k][v], pre, p.act, p.slope);
                     o[v] = rs[v] * (gg - mg[v] - xh * mgx[v]);
                     o2[v] = MODE2 == 2 ? rs2[v] * (gg - mg[v] - xh2 * mgx2[v]) : gg;
                 }

@@ -370,7 +370,9 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
             const float t = __shfl_down_sync(0xffffffffu, inc, o);
             if (lane + o < 32) inc += t;
         }
-        suffix = inc - sumdt;
+        // the right neighbour's inclusive sum, not inc - sumdt: a non-finite dt of this run must not reach its own decay
+        const float right = __shfl_down_sync(0xffffffffu, inc, 1);
+        suffix = lane < 31 ? right : 0.f;
     }
 
     float *rdst = rdst0;
