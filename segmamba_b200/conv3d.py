@@ -26,14 +26,14 @@ _CL = torch.channels_last_3d
 # those that tools/conv3d_bench.py measured to be at least 10 % faster than cuDNN's heuristic plan at batch 2 in bf16 on an
 # H100 80GB HBM3 (700 W).  Every other pass of a routed convolution, and every other convolution, runs on cuDNN.
 NATIVE_PASSES = {
-    (48, 48, 128 ** 3): "fd",
-    (96, 48, 128 ** 3): "f",
-    (48, 48, 64 ** 3): "fd",
-    (48, 96, 64 ** 3): "f",
-    (96, 96, 64 ** 3): "f",
+    (48, 48, 128 ** 3): "fdw",
+    (96, 48, 128 ** 3): "fw",
+    (48, 48, 64 ** 3): "fdw",
+    (48, 96, 64 ** 3): "fw",
+    (96, 96, 64 ** 3): "fw",
     (192, 96, 64 ** 3): "w",
-    (96, 96, 32 ** 3): "f",
-    (96, 192, 32 ** 3): "d",
+    (96, 96, 32 ** 3): "fw",
+    (96, 192, 32 ** 3): "dw",
     (192, 192, 32 ** 3): "d",
     (192, 384, 16 ** 3): "f",
     (384, 384, 16 ** 3): "f",
