@@ -12,7 +12,6 @@ import os
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from . import causal_conv1d_cuda
 from ._lib import DIR_FORWARD, DIR_REVERSE
@@ -21,13 +20,6 @@ from .selective_scan_interface import mamba_inner_fn_no_out_proj
 
 
 # opt-in: run the three directional passes of a mixer on separate CUDA streams (see Mamba.forward)
-def _tc_ok(x2d, weight):
-    """the native GEMM takes 16-bit operands: autocast on, or 16-bit activations; rows must be 16-byte multiples"""
-    cd = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else x2d.dtype
-    return (_gemm.MODE != "off" and x2d.is_cuda and cd in (torch.float16, torch.bfloat16) and x2d.shape[1] % 8 == 0 and weight.shape[0] % 8 == 0
-            and x2d.shape[0] % 8 == 0)
-
-
 DIRECTION_STREAMS = os.environ.get("SMB_DIR_STREAMS", "0") == "1"
 _SIDE_STREAMS = {}
 
@@ -122,11 +114,7 @@ class Mamba(nn.Module):
             raise RuntimeError(f"Mamba v3: seqlen {seqlen} is not divisible by nslices {self.nslices}")
         # matmul and transpose BLH -> HBL at the same time (mamba_simple.py:204-208)
         x2d = hidden_states.reshape(batch * seqlen, -1)
-        tc = _tc_ok(x2d, self.in_proj.weight)                 # 16-bit arithmetic (autocast): the native tensor-core GEMM
-        if tc:
-            xz = _gemm.matmul_nt(self.in_proj.weight, x2d).view(-1, batch, seqlen).permute(1, 0, 2)
-        else:
-            xz = (self.in_proj.weight @ x2d.t()).view(-1, batch, seqlen).permute(1, 0, 2)
+        xz = _gemm.matmul_nt(self.in_proj.weight, x2d).view(-1, batch, seqlen).permute(1, 0, 2)
         if self.in_proj.bias is not None:
             xz = xz + self.in_proj.bias.to(dtype=xz.dtype)[None, :, None]
 
@@ -167,11 +155,12 @@ class Mamba(nn.Module):
             out_b = inner(xz, "_b", DIR_REVERSE)                           # :230-242 without the flip copies
             out_s = slice_pass()
         y = out + out_b + out_s
-        if tc and self.out_proj.bias is None:
-            # (b l, d) x (C, d)^T: y stays in its channel-major storage, it enters the GEMM as an MN-major operand
-            y2d = y.permute(1, 0, 2).reshape(y.shape[1], batch * seqlen)
-            return _gemm.matmul_nt(y2d.t(), self.out_proj.weight).view(batch, seqlen, -1)
-        return F.linear(y.permute(0, 2, 1), self.out_proj.weight, self.out_proj.bias)     # :264
+        # (b l, d) x (C, d)^T (:264): y stays in its channel-major storage, it enters the GEMM as an MN-major operand
+        y2d = y.permute(1, 0, 2).reshape(y.shape[1], batch * seqlen)
+        y = _gemm.matmul_nt(y2d.t(), self.out_proj.weight).view(batch, seqlen, -1)
+        if self.out_proj.bias is not None:
+            y = y + self.out_proj.bias.to(dtype=y.dtype)
+        return y
 
 
 class _SeqPermute(torch.autograd.Function):

@@ -20,7 +20,6 @@ from __future__ import annotations
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from . import gemm as _gemm
 from . import conv3d as _conv3d
@@ -30,20 +29,6 @@ from .instance_norm import fused_instance_norm
 from .mamba_simple import Mamba
 
 _CL = torch.channels_last_3d
-
-def _pointwise(conv: nn.Conv3d, x: torch.Tensor, gelu: bool = False) -> torch.Tensor:
-    """1x1x1 convolution (+ exact GELU) of a channels-last activation.  With 16-bit arithmetic (autocast) it is one
-    (tokens, C_in) x (C_out, C_in)^T product on the native tensor-core GEMM, bias and GELU applied in the accumulator epilogue;
-    in fp32 (no autocast) it stays the library convolution the reference calls (segmamba.py:81-89,103-107)."""
-    cd = torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else x.dtype
-    if (_gemm.MODE == "all" and x.is_cuda and cd in (torch.float16, torch.bfloat16) and conv.kernel_size == (1, 1, 1) and conv.stride == (1, 1, 1)
-            and conv.in_channels % 8 == 0 and conv.out_channels % 8 == 0
-            and x.is_contiguous(memory_format=_CL) and (x.numel() // conv.in_channels) % 8 == 0):
-        if gelu and conv.bias is None:
-            return F.gelu(_gemm.conv1x1(x, conv.weight, None))
-        return _gemm.conv1x1(x, conv.weight, conv.bias, gelu=gelu)
-    y = conv(x)
-    return F.gelu(y) if gelu else y
 
 
 class _ZeroGradBias(torch.autograd.Function):
@@ -66,26 +51,10 @@ def _conv_before_norm(conv: nn.Conv3d, x: torch.Tensor) -> torch.Tensor:
     has passed through the norm -- is analytically zero.  So the bias is neither added (one full-tensor ATen kernel per
     convolution) nor reduced in the backward (one reduction per convolution); the parameter stays in the graph with an exact
     zero gradient, so weight decay acts on it exactly as in the reference and the state_dict surface is unchanged."""
+    entry = _gemm.pointwise_conv if conv.kernel_size == (1, 1, 1) else _conv3d.conv3d
     if conv.bias is None:
-        return _pointwise(conv, x) if conv.kernel_size == (1, 1, 1) else _conv3d.conv3d(conv, x)
-    if conv.kernel_size == (1, 1, 1) and _gemm.MODE == "all":
-        y = _pointwise(_BiasFree(conv), x)
-    else:
-        y = _conv3d.conv3d(conv, x, bias=False)
-    return _ZeroGradBias.apply(y, conv.bias)
-
-
-class _BiasFree:
-    """view of a Conv3d without its bias, for ``_pointwise``"""
-
-    def __init__(self, conv):
-        self.weight, self.bias = conv.weight, None
-        self.kernel_size, self.stride, self.in_channels, self.out_channels = conv.kernel_size, conv.stride, conv.in_channels, conv.out_channels
-        self._conv = conv
-
-    def __call__(self, x):
-        c = self._conv
-        return F.conv3d(x, c.weight, None, c.stride, c.padding, c.dilation, c.groups)
+        return entry(conv, x)
+    return _ZeroGradBias.apply(entry(conv, x, bias=False), conv.bias)
 
 
 class _Conv(nn.Sequential):
@@ -121,7 +90,7 @@ class UnetResBlock(nn.Module):
         out = fused_instance_norm(_conv3d.conv3d(self.conv1.conv, inp), "leaky_relu", 0.01)   # dynunet_block.py:100-102
         out = _conv3d.conv3d(self.conv2.conv, out)
         if self.downsample:                                                               # :105-110
-            return fused_instance_norm(out, "leaky_relu", 0.01, add=_pointwise(self.conv3.conv, inp), add_norm=True)
+            return fused_instance_norm(out, "leaky_relu", 0.01, add=_gemm.pointwise_conv(self.conv3.conv, inp), add_norm=True)
         return fused_instance_norm(out, "leaky_relu", 0.01, add=inp)
 
 
@@ -208,7 +177,7 @@ class MlpChannel(nn.Module):
         self.fc2 = nn.Conv3d(mlp_dim, hidden_size, 1)
 
     def forward(self, x):
-        return _pointwise(self.fc2, _pointwise(self.fc1, x, gelu=True))      # act = exact-erf nn.GELU(), fused into fc1's epilogue
+        return _gemm.pointwise_conv(self.fc2, _gemm.pointwise_conv(self.fc1, x, gelu=True))   # act = exact-erf nn.GELU(), fused into fc1's epilogue
 
 
 class GSC(nn.Module):

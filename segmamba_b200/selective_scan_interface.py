@@ -112,25 +112,6 @@ def causal_conv1d_fn(x, weight, bias=None, activation=None):
     return CausalConv1dFn.apply(x, weight, bias, activation)
 
 
-def _mm_nt(a, b, out=None, accumulate=False, out_dtype=None, split_tokens=0):
-    """a @ b.T for 2-D views.  16-bit operands run on the native tensor-core GEMM (smb_gemm; no operand is copied: a view whose
-    first axis is contiguous goes in MN-major); fp32 operands (the module used without autocast) stay a library call.
-    split_tokens: length of the contraction when it runs over the token axis (weight gradients) -> split-K with fp32 atomics."""
-    native = _gemm.MODE == "all" or (_gemm.MODE == "auto" and split_tokens >= _gemm.SPLIT_TOKENS)
-    if native and a.dtype in (torch.float16, torch.bfloat16) and a.is_cuda and _gemm.supported(a, b):
-        sk = _gemm._split_k_for(split_tokens) if split_tokens >= _gemm.SPLIT_TOKENS else 1
-        od = torch.float32 if sk > 1 else out_dtype
-        return _gemm.gemm(a, b, out=out, accumulate=accumulate, out_dtype=od, split_k=sk)   # split-K results stay fp32
-    res = a @ b.t()
-    if out is not None:
-        if accumulate:
-            out.add_(res)
-        else:
-            out.copy_(res)
-        return out
-    return res
-
-
 def _as_dbl(t):
     """(b, d, l) -> (d, b*l) matrix; a view for the channel-major ("HBL") layout the mixer produces, else one copy."""
     return t.permute(1, 0, 2).reshape(t.shape[1], t.shape[0] * t.shape[2])
@@ -175,8 +156,8 @@ class MambaInnerFnNoOutProj(torch.autograd.Function):
             x_proj_weight = torch.cat([x_proj_weight[:delta_rank], x_proj_weight.new_zeros(R8 - delta_rank, d_inner),
                                        x_proj_weight[delta_rank:]], dim=0)             # (R8+2N, d_inner)
             delta_proj_weight = torch.nn.functional.pad(delta_proj_weight, (0, R8 - delta_rank))   # (d_inner, R8)
-        x_dblT = _mm_nt(x_proj_weight, conv2.t())                                       # (R8+2N, b*l)  = x_dbl.t()   :181
-        delta = _mm_nt(delta_proj_weight, x_dblT[:R8].t()).view(d_inner, bsz, L).permute(1, 0, 2)     # HBL          :182
+        x_dblT = _gemm.product(x_proj_weight, conv2.t())                                # (R8+2N, b*l)  = x_dbl.t()   :181
+        delta = _gemm.product(delta_proj_weight, x_dblT[:R8].t()).view(d_inner, bsz, L).permute(1, 0, 2)     # HBL          :182
         Bm = x_dblT[R8:R8 + d_state].view(d_state, bsz, L).permute(1, 0, 2).unsqueeze(1)                # (b,1,N,l) view
         Cm = x_dblT[R8 + d_state:].view(d_state, bsz, L).permute(1, 0, 2).unsqueeze(1)
         D = D.contiguous() if D is not None else None
@@ -209,7 +190,7 @@ class MambaInnerFnNoOutProj(torch.autograd.Function):
         bsz, d_inner, _ = conv1d_out.shape
         conv2 = _as_dbl(conv1d_out)
         if delta is None:
-            delta = _mm_nt(delta_proj_weight, x_dblT[:R8].t()).view(d_inner, bsz, L).permute(1, 0, 2)
+            delta = _gemm.product(delta_proj_weight, x_dblT[:R8].t()).view(d_inner, bsz, L).permute(1, 0, 2)
         Bm = x_dblT[R8:R8 + d_state].view(d_state, bsz, L).permute(1, 0, 2).unsqueeze(1)
         Cm = x_dblT[R8 + d_state:].view(d_state, bsz, L).permute(1, 0, 2).unsqueeze(1)
         dxz = torch.empty_like(xz)                      # dx and dz are written next to each other (ssi.py:244-245)
@@ -222,12 +203,12 @@ class MambaInnerFnNoOutProj(torch.autograd.Function):
         dx_dblT[R8 + d_state:].view(d_state, bsz, L).copy_(dC.squeeze(1).permute(1, 0, 2))                      # :264-271
         ntok = bsz * L
         ddelta2 = _as_dbl(ddelta)                                                                               # :272
-        ddelta_proj_weight = _mm_nt(ddelta2, x_dblT[:R8], split_tokens=ntok)                                    # :273
+        ddelta_proj_weight = _gemm.product(ddelta2, x_dblT[:R8], ntok)                                          # :273
         # (R8, d) copy of the small weight: as a transposed VIEW its rows would be 16 bytes long, a TMA box shape that crawls
-        _mm_nt(delta_proj_weight.t().contiguous(), ddelta2.t(), out=dx_dblT[:R8])   # rows delta_rank..R8 are exact zeros  :274
+        _gemm.product(delta_proj_weight.t().contiguous(), ddelta2.t(), out=dx_dblT[:R8])   # rows delta_rank..R8 are exact zeros  :274
         dconv2 = _as_dbl(dconv1d_out)                                                                           # :275
-        dx_proj_weight = _mm_nt(dx_dblT, conv2, split_tokens=ntok)                                              # :276
-        dconv2 = _mm_nt(x_proj_weight.t(), dx_dblT.t(), out=dconv2, accumulate=True)                            # :277
+        dx_proj_weight = _gemm.product(dx_dblT, conv2, ntok)                                                    # :276
+        dconv2 = _gemm.product(x_proj_weight.t(), dx_dblT.t(), out=dconv2, accumulate=True)                     # :277
         if R8 != delta_rank:                                          # gradients of the un-padded parameters
             ddelta_proj_weight = ddelta_proj_weight[:, :delta_rank]
             dx_proj_weight = torch.cat([dx_proj_weight[:delta_rank], dx_proj_weight[R8:]], dim=0)
