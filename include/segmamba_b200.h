@@ -23,7 +23,7 @@
  *   smb_conv3d*       the dense 3x3x3 convolutions (cuDNN in the reference): UnetResBlock.conv1 / conv2
  *                     (dynunet_block.py) and GSC.proj / proj2 (segmamba.py)
  *
- * Scope (SURVEY.md section 8): real A, input-dependent ("variable") B and C, dstate in {8, 16},
+ * Scope (SURVEY.md section 8): real A, input-dependent ("variable") B and C, dstate in {8, 16, 32, 64},
  * conv width 2..4, non-channel-last conv layout, fp32 / fp16 / bf16 I/O with fp32 arithmetic.
  * Complex A, constant B/C, channel-last conv and the decode-time `update` kernels are out of scope;
  * calling with them returns SMB_EUNSUPPORTED.

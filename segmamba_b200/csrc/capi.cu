@@ -72,7 +72,7 @@ size_t seg_floats_max(int batch, int dim, int L, int N) {
 
 int check_common(int batch, int dim, int L, int N, int G, int dtype, const char *who) {
     if (batch <= 0 || dim <= 0 || L <= 0) return fail(SMB_EINVAL, "%s: batch, dim and seqlen must be positive", who);
-    if (N != 8 && N != 16) return fail(SMB_EUNSUPPORTED, "%s: dstate %d unsupported (8 or 16)", who, N);
+    if (N != 8 && N != 16 && N != 32 && N != 64) return fail(SMB_EUNSUPPORTED, "%s: dstate %d unsupported (8, 16, 32 or 64)", who, N);
     if (G <= 0 || dim % G != 0) return fail(SMB_EINVAL, "%s: dim %d not divisible by n_groups %d", who, dim, G);
     if (dtype < SMB_F32 || dtype > SMB_BF16) return fail(SMB_EINVAL, "%s: bad dtype %d", who, dtype);
     return SMB_OK;

@@ -428,17 +428,19 @@ __device__ __forceinline__ void prefetch_tiles(const T *const (&bases)[KA], cons
 // ---------------------------------------------------------------------------------------------
 // Warp-private B / C tile: 32 scan positions x N states, position-major so that one position's
 // states are read with broadcast LDS.128 by every lane (lane == channel).  The 16-byte chunk
-// index is XOR-swizzled with (q>>1) to spread the transposing fill over 8 bank groups.
+// index is XOR-swizzled with (q>>1) to spread the transposing fill over 8 bank groups.  The swizzle takes at most two bits of
+// q>>1, so that within a block of 8 positions it depends on the local position alone (bc_read4_c's constant offsets).
 // ---------------------------------------------------------------------------------------------
+template <int N> constexpr int bc_swz() { return N >= 16 ? 3 : N / 4 - 1; }
 template <int N> __device__ __forceinline__ int bc_off(int q, int n) {
-    return q * N + ((((n >> 2) ^ ((q >> 1) & (N / 4 - 1)))) << 2) + (n & 3);
+    return q * N + ((((n >> 2) ^ ((q >> 1) & bc_swz<N>()))) << 2) + (n & 3);
 }
 // same, for a position known at compile time relative to a block of 8 positions (blk = tile + 8*k*N): constant offset
 template <int N, int QL, int CH> __device__ __forceinline__ float4 bc_read4_c(const float *blk) {
-    return *reinterpret_cast<const float4 *>(blk + QL * N + (((CH ^ ((QL >> 1) & (N / 4 - 1)))) << 2));
+    return *reinterpret_cast<const float4 *>(blk + QL * N + (((CH ^ ((QL >> 1) & bc_swz<N>()))) << 2));
 }
 template <int N> __device__ __forceinline__ float4 bc_read4(const float *tile, int q, int chunk) {
-    return *reinterpret_cast<const float4 *>(tile + q * N + (((chunk ^ ((q >> 1) & (N / 4 - 1)))) << 2));
+    return *reinterpret_cast<const float4 *>(tile + q * N + (((chunk ^ ((q >> 1) & bc_swz<N>()))) << 2));
 }
 // base points at (state 0, token 0) of the (dstate, L) slab; ns / ls are the state / token strides.
 template <typename T, int N>
@@ -518,17 +520,21 @@ __device__ __forceinline__ void fill_bc_tiles(float *const (&tiles)[K], const T 
     const int j = j0 + lane;
     const bool valid = j < L;
     const int tok = pos_to_tok(valid ? j : 0, L, reverse);
-    T v[K][N];
+    constexpr int kRound = N > 32 ? 32 : N;      // states per round: at most 2 x 32 loads in flight
 #pragma unroll
-    for (int k = 0; k < K; ++k) {
-        const T *b = bases[k] + (int64_t)tok * ls[k];
+    for (int n0 = 0; n0 < N; n0 += kRound) {
+        T v[K][kRound];
 #pragma unroll
-        for (int n = 0; n < N; ++n) v[k][n] = valid ? b[(int64_t)n * ns[k]] : from_f32<T>(0.f);
-    }
+        for (int k = 0; k < K; ++k) {
+            const T *b = bases[k] + (int64_t)tok * ls[k];
 #pragma unroll
-    for (int k = 0; k < K; ++k) {
+            for (int n = 0; n < kRound; ++n) v[k][n] = valid ? b[(int64_t)(n0 + n) * ns[k]] : from_f32<T>(0.f);
+        }
 #pragma unroll
-        for (int n = 0; n < N; ++n) tiles[k][bc_off<N>(lane, n)] = to_f32<T>(v[k][n]);
+        for (int k = 0; k < K; ++k) {
+#pragma unroll
+            for (int n = 0; n < kRound; ++n) tiles[k][bc_off<N>(lane, n0 + n)] = to_f32<T>(v[k][n]);
+        }
     }
 }
 template <typename T, int N, int K>
@@ -538,6 +544,10 @@ __device__ __forceinline__ void prefetch_bc(const T *const (&bases)[K], const in
         const int lo = reverse ? max(L - j0n - kTile, 0) : j0n;
 #pragma unroll
         for (int k = 0; k < K; ++k) prefetch_l2(bases[k] + (int64_t)lane * ns[k] + (int64_t)lo * ls[k]);
+        if constexpr (N > 32) {
+#pragma unroll
+            for (int k = 0; k < K; ++k) prefetch_l2(bases[k] + (int64_t)(lane + 32) * ns[k] + (int64_t)lo * ls[k]);
+        }
     }
 }
 

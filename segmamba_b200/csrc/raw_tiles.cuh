@@ -95,11 +95,15 @@ template <typename T> __device__ __forceinline__ bool bc_aligned(const T *base, 
 // raw (state-major, token-ascending) staging rows -> position-major fp32 broadcast tile; lane == scan position
 template <typename T, int N, bool kRev> __device__ __forceinline__ void convert_bc(float *tile, const T *raw, int lane) {
     const int src = kRev ? kTile - 1 - lane : lane;
-    T v[N];
+    constexpr int kRound = N > 32 ? 32 : N;      // states per round: bounds the registers of the transposing copy
 #pragma unroll
-    for (int n = 0; n < N; ++n) v[n] = raw[n * kTile + src];
+    for (int n0 = 0; n0 < N; n0 += kRound) {
+        T v[kRound];
 #pragma unroll
-    for (int n = 0; n < N; ++n) tile[bc_off<N>(lane, n)] = to_f32<T>(v[n]);
+        for (int n = 0; n < kRound; ++n) v[n] = raw[(n0 + n) * kTile + src];
+#pragma unroll
+        for (int n = 0; n < kRound; ++n) tile[bc_off<N>(lane, n0 + n)] = to_f32<T>(v[n]);
+    }
 }
 
 // ---- synchronous fill / store of a stage tile for ragged or unaligned tiles (same layout, bounds-checked) ----

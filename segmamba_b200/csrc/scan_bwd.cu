@@ -148,6 +148,11 @@ __global__ void __launch_bounds__(kBwdWarps * 32) scan_bwd_main_kernel(const Sca
     const int L = p.L;
 
     // ---- stage B and C for the chunk: thread t <-> position jc + t; all 2N loads in flight before the first store ----
+    if constexpr (N > 32) {
+        stage_bc_rounds<T, N, kRowPad>(sB, sC, reinterpret_cast<const T *>(p.B) + b * p.B_bs + (int64_t)g * p.B_gs,
+                                       reinterpret_cast<const T *>(p.C) + b * p.C_bs + (int64_t)g * p.C_gs, p.B_ns, p.C_ns, p.B_ls,
+                                       p.C_ls, jc, L, rev, threadIdx.x, pad_pos(threadIdx.x));
+    } else
     {
         const T *Bm = reinterpret_cast<const T *>(p.B) + b * p.B_bs + (int64_t)g * p.B_gs;
         const T *Cm = reinterpret_cast<const T *>(p.C) + b * p.C_bs + (int64_t)g * p.C_gs;
@@ -204,12 +209,20 @@ __global__ void __launch_bounds__(kBwdWarps * 32) scan_bwd_main_kernel(const Sca
     float *myB = slabB + warp * kRowPad + bo;
     float *myC = slabC + warp * kRowPad + bo;
 
-    // per-state scalars of this channel, loaded once: lane n holds (A2, h_in, m_in) of state n, broadcast by shuffle
+    // per-state scalars of this channel, loaded once: lane n & 31 holds (A2, h_in, m_in) of state n, broadcast by shuffle
     float A2_l = 0.f, hin_l = 0.f, min_l = 0.f;
     if (active && lane < N) {
         A2_l = p.A[(int64_t)d * N + lane] * kLog2e;
         hin_l = p.hs[(int64_t)b * p.hs_bs + ((int64_t)chunk * N + lane) * p.dim + d];
         min_l = p.Min[(((int64_t)b * p.nck + chunk) * N + lane) * p.dim + d];
+    }
+    float A2_h = 0.f, hin_h = 0.f, min_h = 0.f;         // states 32..63 (64 states only)
+    if constexpr (N > 32) {
+        if (active) {
+            A2_h = p.A[(int64_t)d * N + 32 + lane] * kLog2e;
+            hin_h = p.hs[(int64_t)b * p.hs_bs + ((int64_t)chunk * N + 32 + lane) * p.dim + d];
+            min_h = p.Min[(((int64_t)b * p.nck + chunk) * N + 32 + lane) * p.dim + d];
+        }
     }
     // item pairs (2j, 2j+1) packed for FFMA2
     float2 dt2[kRun / 2], dtu2[kRun / 2], g2[kRun / 2], sLB2[kRun / 2], sAq2[kRun / 2], yy2[kRun / 2];
@@ -224,9 +237,9 @@ __global__ void __launch_bounds__(kBwdWarps * 32) scan_bwd_main_kernel(const Sca
 #pragma unroll 1
     for (int n = 0; n < N; ++n) {
         float2 dB2[kRun / 2], dC2[kRun / 2];
-        const float A2n = __shfl_sync(0xffffffffu, A2_l, n);
-        const float h_in = __shfl_sync(0xffffffffu, hin_l, n);
-        const float m_in = __shfl_sync(0xffffffffu, min_l, n);
+        const float A2n = state_shfl<N>(A2_l, A2_h, n);
+        const float h_in = state_shfl<N>(hin_l, hin_h, n);
+        const float m_in = state_shfl<N>(min_l, min_h, n);
         if (active) {
             float2 Bv2[kRun / 2], Cv2[kRun / 2];
             {
@@ -743,6 +756,256 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 2) scan_bwd_sweep_kernel(co
     (void)oz;
 }
 
+// More than 16 states (32, 64): the same reverse sweep with the dB / dC transpose in rounds of 16 states per tensor.  Each
+// 4-state chunk is written to the transpose buffer as soon as it is computed and every round is reduced before the next one,
+// so no dB / dC terms stay in registers across rounds; the reduced values leave as one vector atomic per (tensor, state,
+// 4 positions) as above.
+template <typename T, int N, bool kHasZ>
+__global__ void __launch_bounds__(kWarpsPerCta * 32, 2) scan_bwd_sweep_wide_kernel(const ScanP p) {
+    using S = typename StashT<T>::type;
+    static_assert(N % 16 == 0 && N > 16, "dstate");
+    constexpr int kRed = (N + 15) / 16;             // rounds of the dB / dC transpose: 16 states of each tensor per round
+    extern __shared__ __align__(16) float smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int w = blockIdx.x * kWarpsPerCta + warp;
+    if (w >= p.n_work) return;
+    const WorkItem wi = decode_work(p, w);          // S == kCkpt, n_seg == nck
+    const int d = wi.d0 + lane;
+    const bool active = lane < wi.nrows;
+    constexpr int kWarpFloats = 4 * kTile * kTile + 2 * kTile * N + 32 * kTrPitch;
+    float *s_dt = smem + warp * kWarpFloats;
+    float *s_u = s_dt + kTile * kTile;
+    float *s_g = s_u + kTile * kTile;
+    float *s_z = s_g + kTile * kTile;
+    float *s_B = s_z + kTile * kTile;
+    float *s_C = s_B + kTile * N;
+    float *s_tr = s_C + kTile * N;
+
+    float2 A2[N / 2], mu[N / 2], dA2[N / 2], hcur[N / 2];
+#pragma unroll
+    for (int m = 0; m < N / 2; ++m) {
+        A2[m] = active ? f2(p.A[(int64_t)d * N + 2 * m] * kLog2e, p.A[(int64_t)d * N + 2 * m + 1] * kLog2e) : f2(0.f, 0.f);
+        const int64_t o = (((int64_t)wi.b * p.nck + wi.seg) * N + 2 * m) * p.dim + d;
+        mu[m] = active ? f2(p.Min[o], p.Min[o + p.dim]) : f2(0.f, 0.f);
+        dA2[m] = f2(0.f, 0.f);
+    }
+    const float bias = (active && p.delta_bias) ? p.delta_bias[d] : 0.f;
+    const float Dv = (active && p.D) ? p.D[d] : 0.f;
+    float dDacc = 0.f, dbacc = 0.f;
+
+    const T *u = reinterpret_cast<const T *>(p.u) + wi.b * p.u_bs + (int64_t)wi.d0 * p.u_ds;
+    const T *dl = reinterpret_cast<const T *>(p.delta) + wi.b * p.delta_bs + (int64_t)wi.d0 * p.delta_ds;
+    const T *go = reinterpret_cast<const T *>(p.dout) + wi.b * p.dout_bs + (int64_t)wi.d0 * p.dout_ds;
+    const T *z = kHasZ ? reinterpret_cast<const T *>(p.z) + wi.b * p.z_bs + (int64_t)wi.d0 * p.z_ds : nullptr;
+    const T *Bm = reinterpret_cast<const T *>(p.B) + wi.b * p.B_bs + (int64_t)wi.g * p.B_gs;
+    const T *Cm = reinterpret_cast<const T *>(p.C) + wi.b * p.C_bs + (int64_t)wi.g * p.C_gs;
+    T *du = reinterpret_cast<T *>(p.du) + wi.b * p.du_bs + (int64_t)wi.d0 * p.du_ds;
+    T *dde = reinterpret_cast<T *>(p.ddelta) + wi.b * p.ddelta_bs + (int64_t)wi.d0 * p.ddelta_ds;
+    T *dz = kHasZ ? reinterpret_cast<T *>(p.dz) + wi.b * p.dz_bs + (int64_t)wi.d0 * p.dz_ds : nullptr;
+    T *oz = (kHasZ && p.out_z) ? reinterpret_cast<T *>(p.out_z) + wi.b * p.out_z_bs + (int64_t)wi.d0 * p.out_z_ds : nullptr;
+    const int64_t m_stride = p.dim, pos_stride = (int64_t)(N / 2) * p.dim;
+    const S *stash = reinterpret_cast<const S *>(p.stash) + (int64_t)wi.b * p.Lpad * pos_stride + d;
+    // this lane's slot of the cross-channel reduction in round r: lanes 0..15 -> dB state 16 r + lane, lanes 16..31 -> dC state
+    // 16 r + lane - 16
+    float *dBC = ((lane < 16) ? p.dB : p.dC) + (((int64_t)wi.b * p.G + wi.g) * N + (lane & 15)) * (int64_t)p.L;
+    const bool red_slot = (lane & 15) < N;
+    const bool vec_ok = (p.L & 3) == 0 && ((reinterpret_cast<uintptr_t>(p.dB) | reinterpret_cast<uintptr_t>(p.dC)) & 15) == 0;
+
+    const int j_begin = wi.seg * kCkpt;
+    const int j_end = min(p.L, j_begin + kCkpt);
+    const int last_tile = j_begin + ((j_end - j_begin - 1) / kTile) * kTile;
+    const bool fast = stream_aligned(u, p.u_ds, p.L, p.reverse) && stream_aligned(dl, p.delta_ds, p.L, p.reverse) &&
+                      stream_aligned(go, p.dout_ds, p.L, p.reverse) && (!kHasZ || stream_aligned(z, p.z_ds, p.L, p.reverse));
+    const LanePtr<T> lps[4] = {lane_ptr(dl, p.delta_ds, p.L, p.reverse, lane), lane_ptr(u, p.u_ds, p.L, p.reverse, lane),
+                               lane_ptr(go, p.dout_ds, p.L, p.reverse, lane),
+                               lane_ptr(kHasZ ? z : dl, kHasZ ? p.z_ds : p.delta_ds, p.L, p.reverse, lane)};
+    // state at the last position of the walk
+    {
+        const S *sp = stash + (int64_t)(last_tile + kTile - 1) * pos_stride;
+#pragma unroll
+        for (int m = 0; m < N / 2; ++m) hcur[m] = active ? stash_cvt(sp[m * m_stride]) : f2(0.f, 0.f);
+    }
+    for (int j0 = last_tile; j0 >= j_begin; j0 -= kTile) {
+        {
+            constexpr int K = kHasZ ? 4 : 3;
+            float *const tiles[4] = {s_dt, s_u, s_g, s_z};
+            const T *const bases[4] = {dl, u, go, kHasZ ? z : dl};
+            const int64_t strides[4] = {p.delta_ds, p.u_ds, p.dout_ds, kHasZ ? p.z_ds : p.delta_ds};
+            if (fast && j0 + kTile <= p.L) {
+                fill_tiles_fast<T, K, 4>(tiles, lps, wi.nrows, j0, p.reverse, lane);
+            } else {
+                fill_tile<T>(s_dt, dl, p.delta_ds, wi.nrows, j0, p.L, p.reverse, lane);
+                fill_tile<T>(s_u, u, p.u_ds, wi.nrows, j0, p.L, p.reverse, lane);
+                fill_tile<T>(s_g, go, p.dout_ds, wi.nrows, j0, p.L, p.reverse, lane);
+                if (kHasZ) fill_tile<T>(s_z, z, p.z_ds, wi.nrows, j0, p.L, p.reverse, lane);
+            }
+            float *const bt[2] = {s_B, s_C};
+            const T *const bb[2] = {Bm, Cm};
+            const int64_t bns[2] = {p.B_ns, p.C_ns}, bls[2] = {p.B_ls, p.C_ls};
+            fill_bc_tiles<T, N, 2>(bt, bb, bns, bls, j0, p.L, p.reverse, lane);
+            if (j0 - kTile >= j_begin) {
+                prefetch_tiles<T, K, 4>(bases, strides, wi.nrows, j0 - kTile, p.L, p.reverse, lane);
+                prefetch_bc<T, N, 2>(bb, bns, bls, j0 - kTile, p.L, p.reverse, lane);
+            }
+        }
+        __syncwarp();
+        prepass_dt(s_dt, lane, bias, p.softplus, j_end - j0);
+        if (kHasZ) {
+            // g <- dout * silu(z) ;  z-slot <- dout * d silu(z)/dz  (then dz = slot * y);  if out_z is wanted keep silu(z) instead
+#pragma unroll
+            for (int c = 0; c < kTile / 4; ++c) {
+                const float4 g4 = tile_read4(s_g, lane, c), z4 = tile_read4(s_z, lane, c);
+                const float gg[4] = {g4.x, g4.y, g4.z, g4.w}, zz[4] = {z4.x, z4.y, z4.z, z4.w};
+                float gn[4], zc[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const float sg = sigmoidf(zz[e]);
+                    gn[e] = gg[e] * zz[e] * sg;
+                    zc[e] = gg[e] * sg * (1.f + zz[e] * (1.f - sg));
+                }
+                tile_write4(s_g, lane, c, make_float4(gn[0], gn[1], gn[2], gn[3]));
+                tile_write4(s_z, lane, c, make_float4(zc[0], zc[1], zc[2], zc[3]));
+            }
+        }
+        // pull the stash lines of the next (lower) tile into L2 while this one is processed: 8 lines (one per state pair) per
+        // position, lane l covers position l of that tile
+        if (j0 - kTile >= 0 && active) {
+            const S *sp = stash + (int64_t)(j0 - kTile + lane) * pos_stride - lane;      // line start: channel d0
+#pragma unroll
+            for (int m = 0; m < N / 2; ++m) prefetch_l2(sp + m * m_stride);
+        }
+#pragma unroll 1
+        for (int c = kTile / 4 - 1; c >= 0; --c) {            // blocks of 4 positions, descending
+            const float4 d4 = tile_read4(s_dt, lane, c), u4 = tile_read4(s_u, lane, c), g4 = tile_read4(s_g, lane, c);
+            float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (kHasZ) z4 = tile_read4(s_z, lane, c);
+            float4 duv = make_float4(0.f, 0.f, 0.f, 0.f), ddv = duv, dzv = duv, red[kRed];
+#pragma unroll
+            for (int r = 0; r < kRed; ++r) red[r] = duv;
+            const int q0 = 4 * c;
+            const float *blkB = s_B + q0 * N, *blkC = s_C + q0 * N;
+#pragma unroll 1
+            for (int e = 3; e >= 0; --e) {
+                const int pos = j0 + q0 + e;
+                const bool valid = pos < j_end;
+                // h_{t-1}: issue the loads first, consume them at the end of this position
+                S hp[N / 2];
+                {
+                    const S *sp = stash + (int64_t)(pos - 1) * pos_stride;
+#pragma unroll
+                    for (int m = 0; m < N / 2; ++m) hp[m] = (active && pos > 0) ? sp[m * m_stride] : stash_zero<S>();
+                }
+                const float dt = e == 3 ? d4.w : e == 2 ? d4.z : e == 1 ? d4.y : d4.x;
+                const float uv = e == 3 ? u4.w : e == 2 ? u4.z : e == 1 ? u4.y : u4.x;
+                const float g = e == 3 ? g4.w : e == 2 ? g4.z : e == 1 ? g4.y : g4.x;
+                const float zc = e == 3 ? z4.w : e == 2 ? z4.z : e == 1 ? z4.y : z4.x;
+                const float2 dt2 = f2(dt, dt), g2 = f2(g, g), dtu2 = f2(dt * uv, dt * uv);
+                float2 yacc = f2(0.f, 0.f), slb = f2(0.f, 0.f), saq = f2(0.f, 0.f);
+                const int sw = ((q0 + e) >> 1) & bc_swz<N>();      // B/C tile swizzle of this position
+                const float *rowB = blkB + e * N, *rowC = blkC + e * N;
+                float rs[kRed];                                    // this lane's reduced dB / dC of each round
+                // more than 16 states: one transpose round per 16 states, each 4-state chunk goes to shared memory as soon as
+                // it is computed, so no dB / dC terms stay in registers across chunks
+                float *row = s_tr + lane * kTrPitch;
+#pragma unroll
+                for (int r = 0; r < kRed; ++r) {
+#pragma unroll
+                    for (int jr = 0; jr < 4; ++jr) {
+                        const int jn = 4 * r + jr;
+                        const float4 b4 = *reinterpret_cast<const float4 *>(rowB + ((jn ^ sw) << 2));
+                        const float4 c4 = *reinterpret_cast<const float4 *>(rowC + ((jn ^ sw) << 2));
+                        float2 vB[2], vC[2];
+#pragma unroll
+                        for (int hh = 0; hh < 2; ++hh) {
+                            const int m = 2 * jn + hh;
+                            const float2 Bp = hh ? f2(b4.z, b4.w) : f2(b4.x, b4.y);
+                            const float2 Cp = hh ? f2(c4.z, c4.w) : f2(c4.x, c4.y);
+                            const float2 a = ex2x2_mufu(fmul2(dt2, A2[m]));
+                            const float2 lam = ffma2(g2, Cp, mu[m]);
+                            mu[m] = fmul2(a, lam);
+                            yacc = ffma2(Cp, hcur[m], yacc);
+                            vC[hh] = fmul2(g2, hcur[m]);
+                            vB[hh] = fmul2(lam, dtu2);
+                            slb = ffma2(lam, Bp, slb);
+                        }
+                        *reinterpret_cast<float4 *>(row + 4 * jr) = make_float4(vB[0].x, vB[0].y, vB[1].x, vB[1].y);
+                        *reinterpret_cast<float4 *>(row + 16 + 4 * jr) = make_float4(vC[0].x, vC[0].y, vC[1].x, vC[1].y);
+                    }
+                    __syncwarp();
+                    const int col = (lane < 16) ? (lane & 15) : 16 + (lane & 15);
+                    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+                    for (int k = 0; k < 32; k += 4) {
+                        s0 += s_tr[(k + 0) * kTrPitch + col];
+                        s1 += s_tr[(k + 1) * kTrPitch + col];
+                        s2 += s_tr[(k + 2) * kTrPitch + col];
+                        s3 += s_tr[(k + 3) * kTrPitch + col];
+                    }
+                    rs[r] = (s0 + s1) + (s2 + s3);
+                    __syncwarp();
+                }
+#pragma unroll
+                for (int m = 0; m < N / 2; ++m) {
+                    const float2 hpv = stash_cvt(hp[m]);
+                    const float2 qm = fmul2(mu[m], hpv);                // lambda_t a_t h_{t-1}
+                    dA2[m] = ffma2(dt2, qm, dA2[m]);
+                    saq = ffma2(A2[m], qm, saq);
+                    hcur[m] = hpv;
+                }
+                const float y = fmaf(Dv, uv, yacc.x + yacc.y);
+                const float lb = slb.x + slb.y;
+                float ddt = fmaf(uv, lb, kLn2 * (saq.x + saq.y));
+                if (p.softplus) ddt *= sigmoid_of_softplus_inv(dt);
+                ddt = valid ? ddt : 0.f;
+                const float duo = fmaf(dt, lb, Dv * g), dzo = zc * y;
+                dDacc = fmaf(g, uv, dDacc);
+                dbacc += ddt;
+                if (e == 3) { duv.w = duo; ddv.w = ddt; dzv.w = dzo; for (int r = 0; r < kRed; ++r) red[r].w = rs[r]; }
+                else if (e == 2) { duv.z = duo; ddv.z = ddt; dzv.z = dzo; for (int r = 0; r < kRed; ++r) red[r].z = rs[r]; }
+                else if (e == 1) { duv.y = duo; ddv.y = ddt; dzv.y = dzo; for (int r = 0; r < kRed; ++r) red[r].y = rs[r]; }
+                else { duv.x = duo; ddv.x = ddt; dzv.x = dzo; for (int r = 0; r < kRed; ++r) red[r].x = rs[r]; }
+            }
+            // in place: u-slot <- du, dt-slot <- ddelta, z-slot <- dz
+            tile_write4(s_u, lane, c, duv);
+            tile_write4(s_dt, lane, c, ddv);
+            if (kHasZ) tile_write4(s_z, lane, c, dzv);
+            // dB / dC: 4 consecutive positions of this lane's (tensor, state) row
+#pragma unroll
+            for (int r = 0; r < kRed; ++r) {
+            if (red_slot) {
+                const int pos0 = j0 + q0;
+                float *dBCr = dBC + (int64_t)(16 * r) * p.L;
+                if (pos0 + 3 < p.L && vec_ok) {
+                    float *a = dBCr + (p.reverse ? (p.L - 4 - pos0) : pos0);
+                    if (!p.reverse) red_add_v4(a, red[r].x, red[r].y, red[r].z, red[r].w);
+                    else red_add_v4(a, red[r].w, red[r].z, red[r].y, red[r].x);
+                } else {
+                    const float rr[4] = {red[r].x, red[r].y, red[r].z, red[r].w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e)
+                        if (pos0 + e < p.L) atomicAdd(dBCr + pos_to_tok(pos0 + e, p.L, p.reverse), rr[e]);
+                }
+            }
+            }
+        }
+        __syncwarp();
+        store_tile<T>(s_u, du, p.du_ds, wi.nrows, j0, p.L, p.reverse, lane);
+        store_tile<T>(s_dt, dde, p.ddelta_ds, wi.nrows, j0, p.L, p.reverse, lane);
+        if (kHasZ) store_tile<T>(s_z, dz, p.dz_ds, wi.nrows, j0, p.L, p.reverse, lane);
+        __syncwarp();
+    }
+    if (active) {
+#pragma unroll
+        for (int m = 0; m < N / 2; ++m) {
+            atomicAdd(p.dA + (int64_t)d * N + 2 * m, dA2[m].x);
+            atomicAdd(p.dA + (int64_t)d * N + 2 * m + 1, dA2[m].y);
+        }
+        if (p.dD) atomicAdd(p.dD + d, dDacc);
+        if (p.ddelta_bias) atomicAdd(p.ddelta_bias + d, dbacc);
+    }
+    (void)oz;
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -767,8 +1030,13 @@ static cudaError_t launch_bwd(const ScanP &p, cudaStream_t st) {
         SMB_SET_SMEM_ONCE((scan_bwd_stash_kernel<T, N>), smf);
         scan_bwd_stash_kernel<T, N><<<ctas, kWarpsPerCta * 32, smf, st>>>(p); count_launch();
         const size_t smr = (size_t)kWarpsPerCta * (4 * kTile * kTile + 2 * kTile * N + 32 * kTrPitch) * sizeof(float);
-        SMB_SET_SMEM_ONCE((scan_bwd_sweep_kernel<T, N, kHasZ>), smr);
-        scan_bwd_sweep_kernel<T, N, kHasZ><<<ctas, kWarpsPerCta * 32, smr, st>>>(p); count_launch();
+        if constexpr (N > 16) {
+            SMB_SET_SMEM_ONCE((scan_bwd_sweep_wide_kernel<T, N, kHasZ>), smr);
+            scan_bwd_sweep_wide_kernel<T, N, kHasZ><<<ctas, kWarpsPerCta * 32, smr, st>>>(p); count_launch();
+        } else {
+            SMB_SET_SMEM_ONCE((scan_bwd_sweep_kernel<T, N, kHasZ>), smr);
+            scan_bwd_sweep_kernel<T, N, kHasZ><<<ctas, kWarpsPerCta * 32, smr, st>>>(p); count_launch();
+        }
         return cudaGetLastError();
     }
     // R3 (low-memory path; also used when the caller wants out_z recomputed)
@@ -787,8 +1055,12 @@ static cudaError_t launch_bwd(const ScanP &p, cudaStream_t st) {
 
 template <typename T>
 static cudaError_t launch_bwd_t(const ScanP &p, int N, bool has_z, cudaStream_t st) {
-    if (N == 16) return has_z ? launch_bwd<T, 16, true>(p, st) : launch_bwd<T, 16, false>(p, st);
-    return has_z ? launch_bwd<T, 8, true>(p, st) : launch_bwd<T, 8, false>(p, st);
+    switch (N) {
+        case 64: return has_z ? launch_bwd<T, 64, true>(p, st) : launch_bwd<T, 64, false>(p, st);
+        case 32: return has_z ? launch_bwd<T, 32, true>(p, st) : launch_bwd<T, 32, false>(p, st);
+        case 16: return has_z ? launch_bwd<T, 16, true>(p, st) : launch_bwd<T, 16, false>(p, st);
+        default: return has_z ? launch_bwd<T, 8, true>(p, st) : launch_bwd<T, 8, false>(p, st);
+    }
 }
 
 cudaError_t scan_bwd_dispatch(const ScanP &p, int dtype, int N, bool has_z, cudaStream_t st) {

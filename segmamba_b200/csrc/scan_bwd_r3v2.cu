@@ -24,7 +24,8 @@ namespace {
 
 constexpr int kW = 8;                      // channels (warps) per CTA
 constexpr int kPad = kCkpt + 32;           // padded shared row: position p lives at p + (p >> 5) * 4
-constexpr int kDaPitch = 17;               // sDA[warp][lane][state]: pitch coprime with the bank count
+// sDA[warp][lane][state]: partials of up to 32 states (64 states: two passes), pitch coprime with the bank count
+template <int N> constexpr int da_pitch() { return N <= 16 ? 17 : 33; }
 static_assert(kRun * 32 == kCkpt, "R3 chunk must equal the checkpoint interval");
 
 __device__ __forceinline__ int padp(int p) { return p + ((p >> 5) << 2); }
@@ -209,17 +210,18 @@ __device__ __forceinline__ void r3_state(const float *__restrict__ rowB, const f
 template <int N> struct R3Smem {
     static constexpr int kBC = 2 * N * kPad;              // sB, sC
     static constexpr int kSlab = 2 * 2 * kW * kPad;       // [state of the round][tensor][warp][kPad]
-    static constexpr int kDa = kW * 32 * kDaPitch;
+    static constexpr int kDa = kW * 32 * da_pitch<N>();
     static constexpr size_t kBytes = sizeof(float) * (size_t)(kBC + kSlab + kDa);
 };
 
 template <typename T, int N, bool kHasZ, bool kDense>
-__global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP p) {
+__global__ void __launch_bounds__(kW * 32, scan_minb<N>(2)) scan_bwd_main2_kernel(const ScanP p) {
     extern __shared__ __align__(16) float smem[];
     float *sB = smem;                                   // [N][kPad]
     float *sC = sB + N * kPad;                          // [N][kPad]
     float *slab = sC + N * kPad;                        // [2][2][kW][kPad]
-    float *sDA = slab + R3Smem<N>::kSlab;               // [kW][32][kDaPitch]
+    float *sDA = slab + R3Smem<N>::kSlab;               // [kW][32][da_pitch]
+    constexpr int kDaPitch = da_pitch<N>();
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int chunk = blockIdx.x, b = blockIdx.z;
@@ -236,6 +238,11 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
     const int L = p.L;
 
     // ---- stage B and C for the chunk: thread t <-> position jc + t; all 2N loads in flight before the first store ----
+    if constexpr (N > 32) {
+        stage_bc_rounds<T, N, kPad>(sB, sC, reinterpret_cast<const T *>(p.B) + b * p.B_bs + (int64_t)g * p.B_gs,
+                                    reinterpret_cast<const T *>(p.C) + b * p.C_bs + (int64_t)g * p.C_gs, p.B_ns, p.C_ns, p.B_ls, p.C_ls,
+                                    jc, L, rev, threadIdx.x, padp(threadIdx.x));
+    } else
     {
         const T *Bm = reinterpret_cast<const T *>(p.B) + b * p.B_bs + (int64_t)g * p.B_gs;
         const T *Cm = reinterpret_cast<const T *>(p.C) + b * p.C_bs + (int64_t)g * p.C_gs;
@@ -333,13 +340,22 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
         *reinterpret_cast<float4 *>(myC1) = z4; *reinterpret_cast<float4 *>(myC1 + 4) = z4;
     }
 
-    // per-state scalars of this channel, loaded once: lane n holds (A2, h_in, m_in) of state n, broadcast by shuffle
+    // per-state scalars of this channel, loaded once: lane n & 31 holds (A2, h_in, m_in) of state n, broadcast by shuffle
     float A2_l = 0.f, hin_l = 0.f, min_l = 0.f;
     if (active && lane < N) {
         A2_l = p.A[(int64_t)d * N + lane] * kLog2e;
         if (!kDense) hin_l = p.hs[(int64_t)b * p.hs_bs + ((int64_t)chunk * N + lane) * p.dim + d];
         min_l = p.Min[(((int64_t)b * p.nck + chunk) * N + lane) * p.dim + d];
     }
+    float A2_h = 0.f, hin_h = 0.f, min_h = 0.f;         // states 32..63 (64 states only)
+    if constexpr (N > 32) {
+        if (active) {
+            A2_h = p.A[(int64_t)d * N + 32 + lane] * kLog2e;
+            if (!kDense) hin_h = p.hs[(int64_t)b * p.hs_bs + ((int64_t)chunk * N + 32 + lane) * p.dim + d];
+            min_h = p.Min[(((int64_t)b * p.nck + chunk) * N + 32 + lane) * p.dim + d];
+        }
+    }
+    float dA_lo = 0.f;                                  // 64 states: dA of state `lane`, reduced after the first 32 states
     // scan-free path: this lane's own checkpoints (state entering its run; local adjoint entering it from the right, which R1
     // computed with a zero adjoint at the chunk end -- the carried adjoint Min comes in through the decay product below)
     const float *hdp = nullptr, *mdp = nullptr;
@@ -387,9 +403,9 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
     }
 #pragma unroll 1
     for (int n = 0; n < N; n += 2) {
-        const float A2a = __shfl_sync(0xffffffffu, A2_l, n), A2b = __shfl_sync(0xffffffffu, A2_l, n + 1);
-        const float hia = __shfl_sync(0xffffffffu, hin_l, n), hib = __shfl_sync(0xffffffffu, hin_l, n + 1);
-        const float mia = __shfl_sync(0xffffffffu, min_l, n), mib = __shfl_sync(0xffffffffu, min_l, n + 1);
+        const float A2a = state_shfl<N>(A2_l, A2_h, n), A2b = state_shfl<N>(A2_l, A2_h, n + 1);
+        const float hia = state_shfl<N>(hin_l, hin_h, n), hib = state_shfl<N>(hin_l, hin_h, n + 1);
+        const float mia = state_shfl<N>(min_l, min_h, n), mib = state_shfl<N>(min_l, min_h, n + 1);
         if (active && !(p.dbg & 4)) {
             if constexpr (kDense) {
                 const float2 hv = hv_nx, mv = mv_nx;
@@ -398,11 +414,25 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
                     if (use_m) mv_nx = *reinterpret_cast<const float2 *>(mdp + n + 2);
                 }
                 const float ma = fmaf(ex2(A2a * suffix), mia, mv.x), mb = fmaf(ex2(A2b * suffix), mib, mv.y);
-                r3_state<true>(rowB, rowC, A2a, hv.x, ma, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB0, myC0, sda + n);
-                r3_state<true>(rowB + kPad, rowC + kPad, A2b, hv.y, mb, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB1, myC1, sda + n + 1);
+                r3_state<true>(rowB, rowC, A2a, hv.x, ma, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB0, myC0, sda + (N > 32 ? (n & 31) : n));
+                r3_state<true>(rowB + kPad, rowC + kPad, A2b, hv.y, mb, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB1, myC1, sda + (N > 32 ? (n & 31) : n) + 1);
             } else {
-                r3_state<false>(rowB, rowC, A2a, hia, mia, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB0, myC0, sda + n);
-                r3_state<false>(rowB + kPad, rowC + kPad, A2b, hib, mib, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB1, myC1, sda + n + 1);
+                r3_state<false>(rowB, rowC, A2a, hia, mia, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB0, myC0, sda + (N > 32 ? (n & 31) : n));
+                r3_state<false>(rowB + kPad, rowC + kPad, A2b, hib, mib, sumdt, lane, dt2, dtu2, g2, sLB2, sAq2, yy2, myB1, myC1, sda + (N > 32 ? (n & 31) : n) + 1);
+            }
+        }
+        if constexpr (N > 32) {
+            if (n == 30 && active) {                    // states 0..31 complete: free the partial buffer for states 32..63
+                __syncwarp();
+                const float *col = sDA + (warp * 32) * kDaPitch + lane;
+                float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+                for (int k = 0; k < 32; k += 4) {
+                    s0 += col[(k + 0) * kDaPitch]; s1 += col[(k + 1) * kDaPitch];
+                    s2 += col[(k + 2) * kDaPitch]; s3 += col[(k + 3) * kDaPitch];
+                }
+                dA_lo = (s0 + s1) + (s2 + s3);
+                __syncwarp();
             }
         }
         rowB += 2 * kPad; rowC += 2 * kPad;
@@ -447,7 +477,12 @@ __global__ void __launch_bounds__(kW * 32, 2) scan_bwd_main2_kernel(const ScanP 
             s0 += col[(k + 0) * kDaPitch]; s1 += col[(k + 1) * kDaPitch];
             s2 += col[(k + 2) * kDaPitch]; s3 += col[(k + 3) * kDaPitch];
         }
-        atomicAdd(p.dA + (int64_t)d * N + lane, (s0 + s1) + (s2 + s3));
+        if constexpr (N > 32) {
+            atomicAdd(p.dA + (int64_t)d * N + lane, dA_lo);
+            atomicAdd(p.dA + (int64_t)d * N + 32 + lane, (s0 + s1) + (s2 + s3));
+        } else {
+            atomicAdd(p.dA + (int64_t)d * N + lane, (s0 + s1) + (s2 + s3));
+        }
     }
     __syncwarp();                                        // the next octet's partials overwrite these rows
     float sLB[kRun], sAq[kRun], yy[kRun];
@@ -535,8 +570,12 @@ cudaError_t launch_main2(const ScanP &p, cudaStream_t st) {
 }
 template <typename T>
 cudaError_t launch_main2_t(const ScanP &p, int N, bool has_z, cudaStream_t st) {
-    if (N == 16) return has_z ? launch_main2<T, 16, true>(p, st) : launch_main2<T, 16, false>(p, st);
-    return has_z ? launch_main2<T, 8, true>(p, st) : launch_main2<T, 8, false>(p, st);
+    switch (N) {
+        case 64: return has_z ? launch_main2<T, 64, true>(p, st) : launch_main2<T, 64, false>(p, st);
+        case 32: return has_z ? launch_main2<T, 32, true>(p, st) : launch_main2<T, 32, false>(p, st);
+        case 16: return has_z ? launch_main2<T, 16, true>(p, st) : launch_main2<T, 16, false>(p, st);
+        default: return has_z ? launch_main2<T, 8, true>(p, st) : launch_main2<T, 8, false>(p, st);
+    }
 }
 
 }  // namespace

@@ -12,7 +12,7 @@ namespace smb {
 template <int N> struct RaggSmem { static constexpr int kWarpBytes = 6 * kRawTileBytes + kTile * N * 4 + N * kTile * 2; };
 
 template <typename T, int N, bool kHasZ, bool kRev>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, 3) scan_bwd_ragg2_kernel(const ScanP p) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, scan_minb<N>(3)) scan_bwd_ragg2_kernel(const ScanP p) {
     static_assert(sizeof(T) == 2, "the pipelined variant is for 16-bit activations");
     extern __shared__ __align__(16) float smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -133,9 +133,19 @@ static cudaError_t launch_ragg2_n(const ScanP &p, bool has_z, cudaStream_t st) {
     return p.reverse ? launch_ragg2<T, N, false, true>(p, st) : launch_ragg2<T, N, false, false>(p, st);
 }
 
+template <typename T>
+static cudaError_t launch_ragg2_t(const ScanP &p, int N, bool has_z, cudaStream_t st) {
+    switch (N) {
+        case 64: return launch_ragg2_n<T, 64>(p, has_z, st);
+        case 32: return launch_ragg2_n<T, 32>(p, has_z, st);
+        case 16: return launch_ragg2_n<T, 16>(p, has_z, st);
+        default: return launch_ragg2_n<T, 8>(p, has_z, st);
+    }
+}
+
 cudaError_t scan_bwd_ragg_v2_dispatch(const ScanP &p, int dtype, int N, bool has_z, cudaStream_t st) {
-    if (dtype == 1) return N == 16 ? launch_ragg2_n<__half, 16>(p, has_z, st) : launch_ragg2_n<__half, 8>(p, has_z, st);
-    return N == 16 ? launch_ragg2_n<__nv_bfloat16, 16>(p, has_z, st) : launch_ragg2_n<__nv_bfloat16, 8>(p, has_z, st);
+    if (dtype == 1) return launch_ragg2_t<__half>(p, N, has_z, st);
+    return launch_ragg2_t<__nv_bfloat16>(p, N, has_z, st);
 }
 
 }  // namespace smb

@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(1024) carry_kernel(const float *__restrict__ P
 // pass 3
 // ---------------------------------------------------------------------------------------------
 template <typename T, int N, bool kHasZ>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, SMB_FWD_MAIN_MINB) scan_fwd_main_kernel(const ScanP p) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, scan_minb<N>(SMB_FWD_MAIN_MINB)) scan_fwd_main_kernel(const ScanP p) {
     extern __shared__ __align__(16) float smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int w = blockIdx.x * kWarpsPerCta + warp;
@@ -354,8 +354,12 @@ static cudaError_t launch_fwd(const ScanP &p, bool has_z, float *x, cudaStream_t
 
 template <typename T>
 static cudaError_t launch_fwd_n(const ScanP &p, int N, bool has_z, float *x, cudaStream_t st) {
-    if (N == 16) return launch_fwd<T, 16>(p, has_z, x, st);
-    return launch_fwd<T, 8>(p, has_z, x, st);
+    switch (N) {
+        case 64: return launch_fwd<T, 64>(p, has_z, x, st);
+        case 32: return launch_fwd<T, 32>(p, has_z, x, st);
+        case 16: return launch_fwd<T, 16>(p, has_z, x, st);
+        default: return launch_fwd<T, 8>(p, has_z, x, st);
+    }
 }
 
 cudaError_t x_finalize_launch(const ScanP &p, int N, float *x, cudaStream_t st) {
@@ -393,7 +397,9 @@ static cudaError_t launch_agg_only(const ScanP &p, cudaStream_t st) {
 }
 
 cudaError_t scan_fwd_agg_dispatch(const ScanP &p, int dtype, int N, cudaStream_t st) {
-#define SMB_AGG(T) (N == 16 ? launch_agg_only<T, 16>(p, st) : launch_agg_only<T, 8>(p, st))
+#define SMB_AGG(T)                                                                                                  \
+    (N == 64 ? launch_agg_only<T, 64>(p, st) : N == 32 ? launch_agg_only<T, 32>(p, st)                              \
+     : N == 16 ? launch_agg_only<T, 16>(p, st) : launch_agg_only<T, 8>(p, st))
     switch (dtype) {
         case 0: return SMB_AGG(float);
         case 1: return SMB_AGG(__half);

@@ -39,7 +39,7 @@ __device__ __forceinline__ void tma_tile(void *smem, const CUtensorMap *m, int s
 template <int N> struct AggSmem { static constexpr int kWarpBytes = 4 * kRawTileBytes + kTile * N * 4 + N * kTile * 2; };
 
 template <typename T, int N, bool kRev, bool kTma>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, 4) scan_fwd_agg2_kernel(const ScanP p, const __grid_constant__ ScanTmaps tm) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, scan_minb<N>(4)) scan_fwd_agg2_kernel(const ScanP p, const __grid_constant__ ScanTmaps tm) {
     static_assert(sizeof(T) == 2, "the pipelined variant is for 16-bit activations");
     extern __shared__ __align__(1024) float smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(kWarpsPerCta * 32, 4) scan_fwd_agg2_kernel(con
 template <int N> struct MainSmem { static constexpr int kWarpBytes = 6 * kRawTileBytes + 2 * kTile * N * 4 + 2 * N * kTile * 2; };
 
 template <typename T, int N, bool kHasZ, bool kRev, bool kTma>
-__global__ void __launch_bounds__(kWarpsPerCta * 32, 3) scan_fwd_main2_kernel(const ScanP p, const __grid_constant__ ScanTmaps tm) {
+__global__ void __launch_bounds__(kWarpsPerCta * 32, scan_minb<N>(3)) scan_fwd_main2_kernel(const ScanP p, const __grid_constant__ ScanTmaps tm) {
     static_assert(sizeof(T) == 2, "the pipelined variant is for 16-bit activations");
     extern __shared__ __align__(1024) float smem[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -429,9 +429,19 @@ static cudaError_t launch_fwd2_n(const ScanP &p, int dtype, int mode, bool has_z
     return p.reverse ? launch_fwd2<T, N, true, false>(p, tm, has_z, x, st) : launch_fwd2<T, N, false, false>(p, tm, has_z, x, st);
 }
 
+template <typename T>
+static cudaError_t launch_fwd2_t(const ScanP &p, int dtype, int N, int mode, bool has_z, float *x, cudaStream_t st) {
+    switch (N) {
+        case 64: return launch_fwd2_n<T, 64>(p, dtype, mode, has_z, x, st);
+        case 32: return launch_fwd2_n<T, 32>(p, dtype, mode, has_z, x, st);
+        case 16: return launch_fwd2_n<T, 16>(p, dtype, mode, has_z, x, st);
+        default: return launch_fwd2_n<T, 8>(p, dtype, mode, has_z, x, st);
+    }
+}
+
 cudaError_t scan_fwd_v2_dispatch(const ScanP &p, int dtype, int N, bool has_z, float *x, int mode, cudaStream_t st) {
-    if (dtype == 1) return N == 16 ? launch_fwd2_n<__half, 16>(p, dtype, mode, has_z, x, st) : launch_fwd2_n<__half, 8>(p, dtype, mode, has_z, x, st);
-    return N == 16 ? launch_fwd2_n<__nv_bfloat16, 16>(p, dtype, mode, has_z, x, st) : launch_fwd2_n<__nv_bfloat16, 8>(p, dtype, mode, has_z, x, st);
+    if (dtype == 1) return launch_fwd2_t<__half>(p, dtype, N, mode, has_z, x, st);
+    return launch_fwd2_t<__nv_bfloat16>(p, dtype, N, mode, has_z, x, st);
 }
 
 }  // namespace smb

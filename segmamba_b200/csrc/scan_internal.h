@@ -16,6 +16,9 @@ namespace smb {
 #define SMB_FWD_MAIN_MINB 3
 #endif
 constexpr int kWarpsPerCta = SMB_WARPS_PER_CTA;   // independent warps per CTA in the lane-per-channel kernels
+// Minimum resident CTAs per SM asked of ptxas (it sets the register cap).  8 and 16 states keep the tuned value; at 32 / 64 states a
+// lane holds 2-4x the state, and the per-warp shared tiles grow with N so that they bound the residency before registers do.
+template <int N> constexpr int scan_minb(int tuned) { return N <= 16 ? tuned : (N == 32 && tuned > 2 ? 2 : 1); }
 
 struct ScanP {
     int batch, dim, L, G;
@@ -58,6 +61,35 @@ template <int N>
 __device__ __forceinline__ void dense_store(float *dst, const float2 (&v)[N / 2]) {
 #pragma unroll
     for (int k = 0; k < N / 4; ++k) *reinterpret_cast<float4 *>(dst + 4 * k) = make_float4(v[2 * k].x, v[2 * k].y, v[2 * k + 1].x, v[2 * k + 1].y);
+}
+
+// Per-state scalar of one channel held across a warp: state n lives in lane n & 31 of `lo` (n < 32) or `hi` (64 states)
+template <int N> __device__ __forceinline__ float state_shfl(float lo, float hi, int n) {
+    if constexpr (N > 32) return __shfl_sync(0xffffffffu, n < 32 ? lo : hi, n & 31);
+    else return __shfl_sync(0xffffffffu, lo, n);
+}
+// B / C staging of the warp-per-channel R3 kernels for more than 32 states: thread t <-> position jc + t, states in rounds of 32 so
+// that at most 2 x 32 loads are in flight (32 states and fewer stage in one round, inline in the kernels)
+template <typename T, int N, int kPitch>
+__device__ __forceinline__ void stage_bc_rounds(float *sB, float *sC, const T *Bm, const T *Cm, int64_t B_ns, int64_t C_ns, int64_t B_ls,
+                                                int64_t C_ls, int jc, int L, bool rev, int t, int so) {
+    const int j = jc + t;
+    const bool valid = j < L;
+    const int tok = pos_to_tok(valid ? j : 0, L, rev);
+#pragma unroll
+    for (int n0 = 0; n0 < N; n0 += 32) {
+        T vb[32], vc[32];
+#pragma unroll
+        for (int n = 0; n < 32; ++n) {
+            vb[n] = valid ? Bm[(int64_t)(n0 + n) * B_ns + (int64_t)tok * B_ls] : from_f32<T>(0.f);
+            vc[n] = valid ? Cm[(int64_t)(n0 + n) * C_ns + (int64_t)tok * C_ls] : from_f32<T>(0.f);
+        }
+#pragma unroll
+        for (int n = 0; n < 32; ++n) {
+            sB[(n0 + n) * kPitch + so] = to_f32<T>(vb[n]);
+            sC[(n0 + n) * kPitch + so] = to_f32<T>(vc[n]);
+        }
+    }
 }
 
 struct WorkItem {

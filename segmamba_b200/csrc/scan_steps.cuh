@@ -19,14 +19,13 @@ __device__ __forceinline__ void scan_step_agg_chunk(const float *s_B, float2 dt2
     h[2 * JN] = ffma2(a0, h[2 * JN], fmul2(du2, f2(b4.x, b4.y)));
     h[2 * JN + 1] = ffma2(a1, h[2 * JN + 1], fmul2(du2, f2(b4.z, b4.w)));
 }
-template <int N, int QL>
+// chunks JN .. N/4 - 1 of one position, in ascending order
+template <int N, int QL, int JN = 0>
 __device__ __forceinline__ void scan_step_agg(const float *s_B, float2 dt2, float2 du2, const float2 (&A2)[N / 2],
                                               float2 (&h)[N / 2]) {
-    scan_step_agg_chunk<N, QL, 0>(s_B, dt2, du2, A2, h);
-    scan_step_agg_chunk<N, QL, 1>(s_B, dt2, du2, A2, h);
-    if (N == 16) {
-        scan_step_agg_chunk<N, QL, (N == 16 ? 2 : 0)>(s_B, dt2, du2, A2, h);
-        scan_step_agg_chunk<N, QL, (N == 16 ? 3 : 1)>(s_B, dt2, du2, A2, h);
+    if constexpr (JN < N / 4) {
+        scan_step_agg_chunk<N, QL, JN>(s_B, dt2, du2, A2, h);
+        scan_step_agg<N, QL, JN + 1>(s_B, dt2, du2, A2, h);
     }
 }
 template <int N, int QL, int JN>
@@ -41,16 +40,20 @@ __device__ __forceinline__ void scan_step_main_chunk(const float *s_B, const flo
     y = ffma2(f2(c4.x, c4.y), h[2 * JN], y);
     y = ffma2(f2(c4.z, c4.w), h[2 * JN + 1], y);
 }
+// chunks JN .. N/4 - 1 of one position; even chunks accumulate C h into ya, odd ones into yb
+template <int N, int QL, int JN>
+__device__ __forceinline__ void scan_step_main_from(const float *s_B, const float *s_C, float2 dt2, float2 du2,
+                                                    const float2 (&A2)[N / 2], float2 (&h)[N / 2], float2 &ya, float2 &yb) {
+    if constexpr (JN < N / 4) {
+        scan_step_main_chunk<N, QL, JN>(s_B, s_C, dt2, du2, A2, h, (JN & 1) ? yb : ya);
+        scan_step_main_from<N, QL, JN + 1>(s_B, s_C, dt2, du2, A2, h, ya, yb);
+    }
+}
 template <int N, int QL>
 __device__ __forceinline__ float scan_step_main(const float *s_B, const float *s_C, float2 dt2, float2 du2,
                                                 const float2 (&A2)[N / 2], float2 (&h)[N / 2]) {
     float2 ya = f2(0.f, 0.f), yb = f2(0.f, 0.f);
-    scan_step_main_chunk<N, QL, 0>(s_B, s_C, dt2, du2, A2, h, ya);
-    scan_step_main_chunk<N, QL, 1>(s_B, s_C, dt2, du2, A2, h, yb);
-    if (N == 16) {
-        scan_step_main_chunk<N, QL, (N == 16 ? 2 : 0)>(s_B, s_C, dt2, du2, A2, h, ya);
-        scan_step_main_chunk<N, QL, (N == 16 ? 3 : 1)>(s_B, s_C, dt2, du2, A2, h, yb);
-    }
+    scan_step_main_from<N, QL, 0>(s_B, s_C, dt2, du2, A2, h, ya, yb);
     const float2 ys = fadd2(ya, yb);
     return ys.x + ys.y;
 }
@@ -90,14 +93,12 @@ __device__ __forceinline__ void ragg_step_chunk(const float *s_C, float2 dt2, fl
     mu[2 * JN] = fmul2(a0, ffma2(g2, f2(c4.x, c4.y), mu[2 * JN]));
     mu[2 * JN + 1] = fmul2(a1, ffma2(g2, f2(c4.z, c4.w), mu[2 * JN + 1]));
 }
-template <int N, int QL>
+template <int N, int QL, int JN = 0>
 __device__ __forceinline__ void ragg_step(const float *s_C, float2 dt2, float2 g2, const float2 (&A2)[N / 2],
                                           float2 (&mu)[N / 2]) {
-    ragg_step_chunk<N, QL, 0>(s_C, dt2, g2, A2, mu);
-    ragg_step_chunk<N, QL, 1>(s_C, dt2, g2, A2, mu);
-    if (N == 16) {
-        ragg_step_chunk<N, QL, (N == 16 ? 2 : 0)>(s_C, dt2, g2, A2, mu);
-        ragg_step_chunk<N, QL, (N == 16 ? 3 : 1)>(s_C, dt2, g2, A2, mu);
+    if constexpr (JN < N / 4) {
+        ragg_step_chunk<N, QL, JN>(s_C, dt2, g2, A2, mu);
+        ragg_step<N, QL, JN + 1>(s_C, dt2, g2, A2, mu);
     }
 }
 // 8 consecutive positions walked in descending order (compile-time local index QL = 7..0)

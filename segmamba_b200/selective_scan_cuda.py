@@ -65,6 +65,21 @@ def _ws(nbytes, device):
 # main pass starts every 8-position run from a saved state and a saved local adjoint instead of linking the runs with two
 # 5-step warp scans per state.  DENSE_STATES=False keeps the 256-position checkpoints only (A/B; both paths are parity-tested).
 DENSE_STATES = True
+# Dense checkpoints take N / 2 bytes per (position, channel), and the backward allocates as much again for the local adjoints: a
+# call keeps them while that pair stays within DENSE_SHARE of the device's memory, and otherwise runs the backward on the
+# 256-position checkpoints alone.  At 64 states the stage-0 mixer call (batch 2, 96 channels, 262144 positions) needs 3.2 GB, which
+# an 80 GB device keeps dense.
+DENSE_SHARE = 1 / 16
+_DEVICE_BYTES: dict[int, int] = {}
+
+
+def _dense_fits(nfloats, dev):
+    if dev.type != "cuda":
+        return True
+    idx = dev.index if dev.index is not None else torch.cuda.current_device()
+    if idx not in _DEVICE_BYTES:
+        _DEVICE_BYTES[idx] = torch.cuda.get_device_properties(idx).total_memory
+    return 2 * 4 * nfloats <= DENSE_SHARE * _DEVICE_BYTES[idx]
 
 
 def fwd_ex(u, delta, A, B, C, D_=None, z_=None, delta_bias_=None, delta_softplus=False, *, direction=0,
@@ -84,7 +99,9 @@ def fwd_ex(u, delta, A, B, C, D_=None, z_=None, delta_bias_=None, delta_softplus
         l = _lib.lib()
         hdense = None
         if want_hdense and DENSE_STATES:
-            hdense = torch.empty(l.smb_scan_dense_floats(batch, dim, L, N, G), dtype=torch.float32, device=dev)
+            nd = l.smb_scan_dense_floats(batch, dim, L, N, G)
+            if _dense_fits(nd, dev):
+                hdense = torch.empty(nd, dtype=torch.float32, device=dev)
         wsb = l.smb_scan_fwd_workspace_bytes(batch, dim, L, N)
         ws = _ws(wsb, dev)
         a = _lib.ScanFwdArgs()
